@@ -40,7 +40,7 @@ struct GemmParams {
   int chunks_per_tap;       // K chunks per tap (= k_chunks when num_taps == 1)
   int num_taps;
   int tap_shift[9];         // A row shift per tap (3x3 conv over the flattened padded image)
-  int groups;               // blockIdx.z
+  int groups;               // independent GEMMs of one launch (gemm_tile orders their tiles)
   int a_row_group_off, a_col_group_off, a_col_base;   // A coordinates added per group
   int b_row_group_off;      // B rows added per group (usually N)
   int act;

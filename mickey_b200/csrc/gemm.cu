@@ -2,6 +2,7 @@
 #include "gemm.h"
 #include "gemm_tc.cuh"
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
@@ -114,7 +115,8 @@ gemm_simt_kernel(const __half* __restrict__ A, long long a_rows, long long lda, 
   __shared__ __half Bs[BN][BLOCK_K + 8];
   pdl_trigger();
   pdl_wait();
-  const int g = blockIdx.z, m0 = blockIdx.x * BLOCK_M, n0 = blockIdx.y * BN;
+  const GemmTile tile = gemm_tile<BN>(p, blockIdx.x);
+  const int g = tile.g, m0 = tile.m0, n0 = tile.n0;
   const int t = threadIdx.x;
   float acc[BN];
 #pragma unroll
@@ -185,40 +187,6 @@ static bool use_simt() {
   return v == 1;
 }
 
-template <int BN, int EPI, int STAGES>
-static int launch_tc(dim3 grid, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream,
-                     const OutMaps& om = no_out_maps()) {
-  static unsigned long long attr_mask = 0;
-  constexpr int smem = gemm_smem_bytes<BN, EPI, STAGES>();
-  static_assert(smem <= 227 * 1024, "GEMM: shared memory");
-  if (first_use_on_device(attr_mask)) {
-    MK_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  }
-  MK_CUDA_CHECK(launch_k(gemm_tc_kernel<BN, EPI, STAGES>, grid, dim3(GEMM_THREADS), (size_t)smem, stream, tmA, tmB, p, om));
-  return MK_OK;
-}
-
-// EPI_RESID_LN: the grid.y CTAs of a row of tiles form one thread-block cluster (row statistics through DSMEM)
-template <int BN, int EPI, int STAGES>
-static int launch_tc_cluster(dim3 grid, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
-  static unsigned long long attr_mask = 0;
-  constexpr int smem = gemm_smem_bytes<BN, EPI, STAGES>();
-  if (first_use_on_device(attr_mask)) {
-    MK_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = grid.y; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  MK_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, EPI, STAGES>, tmA, tmB, p, no_out_maps()));
-  return MK_OK;
-}
-
 static int sm_count() {
   static int n[64] = {0};
   int dev = 0;
@@ -228,23 +196,55 @@ static int sm_count() {
   return c;
 }
 
-// Ring depth: grids of at most ~one CTA per SM take a deep ring (one CTA per SM, more bytes in flight); bigger grids
-// keep the 96 KB ring, which leaves room for two CTAs per SM.
-template <int BN> constexpr int shallow_stages() { return BN == 128 ? 3 : 4; }
-template <int BN> constexpr int deep_stages() { return BN == 128 ? 6 : 8; }
-static bool deep_ring(const dim3& grid, const GemmParams& p) {
-  return (long long)grid.x * grid.y * grid.z <= (long long)sm_count() * 5 / 4 && p.k_chunks > 3;
+// Persistent instantiations get one CTA per SM (fewer if there are fewer tiles); the one-tile-per-CTA ones one CTA per
+// tile.  EPI_RESID_LN: each row of tiles (gemm_tile keeps it consecutive) forms one thread-block cluster, which
+// exchanges row statistics through DSMEM.
+template <int BN, int EPI, int STAGES, bool PERSISTENT>
+static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream,
+                     const OutMaps& om = no_out_maps()) {
+  static unsigned long long attr_mask = 0;
+  constexpr int smem = gemm_smem_bytes<BN, EPI, STAGES, PERSISTENT>();
+  if (first_use_on_device(attr_mask)) {
+    MK_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, STAGES, PERSISTENT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  }
+  const int tiles = gemm_tile_count<BN>(p);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(PERSISTENT ? std::min(tiles, sm_count()) : tiles);
+  cfg.blockDim = dim3(gemm_threads<PERSISTENT>()); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cudaLaunchAttribute attr[2];
+  int n_attr = 0;
+  if (pdl_enabled()) {
+    attr[n_attr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n_attr++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if constexpr (EPI == EPI_RESID_LN) {
+    attr[n_attr].id = cudaLaunchAttributeClusterDimension;
+    attr[n_attr].val.clusterDim.x = p.N / BN; attr[n_attr].val.clusterDim.y = 1; attr[n_attr++].val.clusterDim.z = 1;
+  }
+  cfg.attrs = attr;
+  cfg.numAttrs = n_attr;
+  MK_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, EPI, STAGES, PERSISTENT>, tmA, tmB, p, om));
+  return MK_OK;
 }
+
+// Grids of at most ~1.25 tiles per SM run one tile per CTA on a deep ring (more bytes in flight per tile).  Grids of more
+// than 8 tiles per SM run the persistent kernel: every ViT-B GEMM and head GEMM of the 32-pair batch (>= 1060 M-tiles).
+// The ones in between run one tile per CTA with two CTAs per SM: every GEMM of a single ViT-S pair (at most 544 tiles),
+// where the persistent kernel measured slower.
+static bool deep_ring(int tiles, const GemmParams& p) {
+  return (long long)tiles <= (long long)sm_count() * 5 / 4 && p.k_chunks > 3;
+}
+static bool persistent_grid(int tiles) { return tiles > 8 * sm_count(); }
 
 template <int BN, int EPI>
 static int launch_one(const GemmOperand& A, const GemmOperand& B, const GemmParams& p, cudaStream_t stream, int impl) {
-  dim3 grid(ceil_div(p.M, BLOCK_M), ceil_div(p.N, BN), p.groups);
+  const int tiles = gemm_tile_count<BN>(p);
   if constexpr (EPI == EPI_RESID_LN) {
-    if (impl == GEMM_IMPL_SIMT || BN != 128 || grid.y > 8 || grid.z != 1) { set_last_error("EPI_RESID_LN: wgmma path, N <= 1024, one group"); return MK_ERR_UNSUPPORTED; }
+    if (impl == GEMM_IMPL_SIMT || BN != 128 || p.N / BN > 8 || p.groups != 1) { set_last_error("EPI_RESID_LN: wgmma path, N <= 1024, one group"); return MK_ERR_UNSUPPORTED; }
   }
   if (impl == GEMM_IMPL_SIMT) {
     if constexpr (EPI != EPI_RESID_LN)
-    MK_CUDA_CHECK(launch_k(gemm_simt_kernel<BN, EPI>, grid, dim3(128), 0, stream, reinterpret_cast<const __half*>(A.ptr),
+    MK_CUDA_CHECK(launch_k(gemm_simt_kernel<BN, EPI>, dim3(tiles), dim3(128), 0, stream, reinterpret_cast<const __half*>(A.ptr),
                            (long long)A.rows, (long long)A.ld, reinterpret_cast<const __half*>(B.ptr), (long long)B.rows,
                            (long long)B.ld, p));
   } else {
@@ -260,16 +260,13 @@ static int launch_one(const GemmOperand& A, const GemmOperand& B, const GemmPara
         float* outs[3] = {p.scores, p.kp_scores, p.final_scores};
         for (int i = 0; i < 3; ++i)
           if (outs[i]) { rc = encode_tensor_map_out_f32(&om.m[i], outs[i], p.n_valid, p.out_pitch, p.groups); if (rc) return rc; }
-        return launch_tc<BN, EPI, shallow_stages<BN>()>(grid, tmA, tmB, p, stream, om);
+        return launch_tc<BN, EPI, shallow_stages<BN>(), false>(tmA, tmB, p, stream, om);
       }
     }
-    const bool deep = deep_ring(grid, p);
-    if constexpr (EPI == EPI_RESID_LN) {
-      if (deep) return launch_tc_cluster<BN, EPI, deep_stages<BN>()>(grid, tmA, tmB, p, stream);
-      return launch_tc_cluster<BN, EPI, shallow_stages<BN>()>(grid, tmA, tmB, p, stream);
-    }
-    if (deep) return launch_tc<BN, EPI, deep_stages<BN>()>(grid, tmA, tmB, p, stream);
-    return launch_tc<BN, EPI, shallow_stages<BN>()>(grid, tmA, tmB, p, stream);
+    if (deep_ring(tiles, p)) return launch_tc<BN, EPI, deep_stages<BN>(), false>(tmA, tmB, p, stream);
+    if constexpr (persistent_epilogue<EPI>())
+      if (persistent_grid(tiles)) return launch_tc<BN, EPI, ring_stages<BN>(), true>(tmA, tmB, p, stream);
+    return launch_tc<BN, EPI, shallow_stages<BN>(), false>(tmA, tmB, p, stream);
   }
   MK_CUDA_CHECK(cudaGetLastError());
   return MK_OK;

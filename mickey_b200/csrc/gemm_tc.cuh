@@ -2,14 +2,23 @@
 //
 //   D[M,N] (fp32) = A[M,K] * B[N,K]^T,   A and B fp16, K-major, 128-byte swizzled tiles
 //
-// CTA = one 128 x BN output tile, 288 threads:
-//   warps 0-3 : consumer warpgroup 0 (wgmma m64nBNk16 on tile rows 0..63)
-//   warps 4-7 : consumer warpgroup 1 (rows 64..127)
-//   warp 8    : TMA producer (one elected lane issues cp.async.bulk.tensor.2d into the smem ring)
-// The accumulators live in the consumers' registers.  When the K loop has drained, the ring is idle and the consumers
-// park the fp32 tile in it, as eight 32 x (BN/2) blocks (the layout epilogue_rows reads), and then run the epilogue:
-// warp w owns rows 32(w&3)..+31 and the column half w>>2.  With the 3-stage ring (96 KB) two CTAs are resident per SM,
-// so one CTA's epilogue overlaps the other's main loop.
+// Output tiles are 128 x BN; every launch walks them in gemm_tile() order.  The persistent instantiations (PERSISTENT,
+// large grids) have 640 threads (five warpgroups) in three roles:
+//   warps 0-7  : MMA warpgroups 0 and 1 (wgmma m64nBNk16 on tile rows 0..63 / 64..127, fp32 accumulators in registers)
+//   warps 8-15 : epilogue warps; warp 8 + w owns rows 32(w&3)..+31 and the column half w>>2 of the tile
+//   warps 16-19: producer warpgroup; one elected lane of warp 16 issues cp.async.bulk.tensor.2d into the smem ring
+// A grid of at most one CTA per SM strides through the tiles by gridDim.x.  The producer's ring stage and phase carry
+// over from tile to tile, so the next tile's loads are in flight while the current one is still in its MMAs.  When a
+// tile's K loop has drained, the MMA warpgroups park the accumulators in a staging buffer outside the ring, as eight
+// 32 x (BN/2) blocks (the layout epilogue_rows reads), and go on to the next tile while the epilogue warps run
+// tile_epilogue from the staged blocks.
+//
+// The other instantiations (!PERSISTENT) run one tile per CTA (grid = tiles, the same loop runs once) with 288 threads:
+// the MMA warps park the accumulators in the idle ring and run the epilogue themselves, warp 8 is the producer.  They
+// serve EPI_DUAL (its TMA-store staging takes the room of a second buffer), EPI_RESID_LN (a thread-block cluster is one
+// row of tiles), EPI_LN (its epilogue needs more registers than the persistent epilogue warps have) and grids too small
+// to keep a persistent CTA per SM busy: a 3-stage ring (two CTAs per SM, one CTA's epilogue under the other's main loop,
+// except for the LayerNorm epilogues) or, for at most ~1.25 tiles per SM, a deep ring.
 //
 // The K loop walks `k_chunks` 64-element chunks.  For convolutions a chunk also selects a filter tap:
 // the A tile of tap t is the same 2-D tensor read at row offset tap_shift[t] (negative / overflowing
@@ -24,8 +33,16 @@ namespace mk {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;        // 64 fp16 = 128 bytes = one swizzle row
 constexpr int WGMMA_K = 16;
-constexpr int GEMM_THREADS = 288;
-constexpr int GEMM_WARP_TMA = 8;
+constexpr int GEMM_WARP_EPI = 8;
+
+// Ring depths: the persistent kernel's ring shares shared memory with the accumulator staging buffer; the one-tile rings
+// have the whole region to themselves.
+template <int BN> constexpr int ring_stages() { return BN == 128 ? 4 : 6; }
+template <int BN> constexpr int shallow_stages() { return BN == 128 ? 3 : 4; }
+template <int BN> constexpr int deep_stages() { return BN == 128 ? 6 : 8; }
+template <int EPI> constexpr bool persistent_epilogue() { return EPI != EPI_DUAL && EPI != EPI_RESID_LN && EPI != EPI_LN; }
+template <bool PERSISTENT> constexpr int gemm_threads() { return PERSISTENT ? 640 : 288; }
+template <bool PERSISTENT> constexpr int gemm_warp_tma() { return PERSISTENT ? 16 : 8; }
 
 // Per-warp staging of EPI_DUAL: three 32 x 32 fp32 boxes (1024-byte aligned) for the TMA stores + 64 floats of column
 // operands (the st.global path uses the first box as its [32][33] transpose buffer)
@@ -36,16 +53,48 @@ constexpr int DUAL_BYTES = 8 * DUAL_STAGE_BYTES + DUAL_AUX_BYTES;
 template <int BN> constexpr int acc_block_floats() { return 32 * (BN / 2 + 4); }   // one warp's 32 x (BN/2) block, ld BN/2 + 4
 template <int BN> constexpr int acc_tile_bytes() { return 8 * acc_block_floats<BN>() * 4; }
 template <int BN, int STAGES> constexpr int ring_bytes() { return STAGES * (BLOCK_M * BLOCK_K * 2 + BN * BLOCK_K * 2); }
-// After the K loop the ring region holds [EPI_DUAL staging][accumulator tile]
-template <int BN, int EPI> constexpr int acc_tile_offset() { return EPI == EPI_DUAL ? DUAL_BYTES : 0; }
-template <int BN, int EPI, int STAGES>
+// Persistent: the accumulator staging buffer follows the ring.  One tile per CTA: after the K loop the ring region
+// holds [EPI_DUAL staging][accumulator tile].
+template <int BN, int EPI, int STAGES, bool PERSISTENT> constexpr int acc_tile_offset() {
+  return PERSISTENT ? ring_bytes<BN, STAGES>() : EPI == EPI_DUAL ? DUAL_BYTES : 0;
+}
+template <int BN, int EPI, int STAGES, bool PERSISTENT>
 constexpr int region_bytes() {
-  return ring_bytes<BN, STAGES>() > acc_tile_offset<BN, EPI>() + acc_tile_bytes<BN>() ? ring_bytes<BN, STAGES>()
-                                                                                       : acc_tile_offset<BN, EPI>() + acc_tile_bytes<BN>();
+  return ring_bytes<BN, STAGES>() > acc_tile_offset<BN, EPI, STAGES, PERSISTENT>() + acc_tile_bytes<BN>()
+             ? ring_bytes<BN, STAGES>() : acc_tile_offset<BN, EPI, STAGES, PERSISTENT>() + acc_tile_bytes<BN>();
 }
 // + 1024 alignment slack + 256 barriers + 2 KB row statistics (EPI_RESID_LN)
-template <int BN, int EPI, int STAGES> constexpr int gemm_smem_bytes() { return region_bytes<BN, EPI, STAGES>() + 1024 + 256 + 2048; }
-template <int BN, int EPI, int STAGES> constexpr int gemm_ctas_per_sm() { return gemm_smem_bytes<BN, EPI, STAGES>() <= 113 * 1024 ? 2 : 1; }
+template <int BN, int EPI, int STAGES, bool PERSISTENT> constexpr int gemm_smem_bytes() {
+  return region_bytes<BN, EPI, STAGES, PERSISTENT>() + 1024 + 256 + 2048;
+}
+// Two one-tile CTAs per SM when their shared memory allows it, except for the LayerNorm epilogues: at two CTAs per SM
+// a thread has 96 registers, and they spill below about 140.
+template <int BN, int EPI, int STAGES, bool PERSISTENT> constexpr int gemm_ctas_per_sm() {
+  return !PERSISTENT && EPI != EPI_LN && EPI != EPI_RESID_LN && gemm_smem_bytes<BN, EPI, STAGES, PERSISTENT>() <= 113 * 1024 ? 2 : 1;
+}
+
+// ---- tile order ----------------------------------------------------------------------------------------
+// Linear tile index -> (group, m0, n0, n_tile).  N-tiles vary fastest, then the groups if they all read the same A
+// rows and columns, then the M-tiles; groups with their own A (matcher pairs, heads with per-group input columns) are
+// outermost, so a group's tiles stay together.  The ViT GEMMs have M in the ~1000 tiles and A far larger than the
+// 50 MB L2 while all of B is a few MB: the ~132 tiles in flight at once then cover a few complete rows of tiles, every
+// A row-panel is read from HBM about once and B stays resident in L2.  An M-fastest order would instead stream A once
+// per column of N-tiles.  EPI_RESID_LN relies on a row of tiles being consecutive: its clusters are those rows.
+struct GemmTile { int g, m0, n0, n_tile; };
+template <int BN>
+__host__ __device__ __forceinline__ int gemm_tile_count(const GemmParams& p) {
+  return ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BN - 1) / BN) * p.groups;
+}
+template <int BN>
+__device__ __forceinline__ GemmTile gemm_tile(const GemmParams& p, int t) {
+  const int n_tiles = (p.N + BN - 1) / BN, m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int n = t % n_tiles;
+  t /= n_tiles;
+  int g, m;
+  if (p.a_row_group_off == 0 && p.a_col_group_off == 0) { g = t % p.groups; m = t / p.groups; }
+  else { m = t % m_tiles; g = t / m_tiles; }
+  return {g, m * BLOCK_M, n * BN, n};
+}
 
 // ---- PTX wrappers ------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -85,7 +134,14 @@ __device__ __forceinline__ bool elect_one() {
       "}" : "=r"(pred));
   return pred != 0;
 }
-// named barrier of the 256 consumer threads (id 1; id 0 is __syncthreads)
+// Warpgroup register budgets of the persistent kernel (setmaxnreg): 640 threads start at 96 registers; the producer warpgroup drops to 40 so that
+// the epilogue warpgroups can hold 120, the MMA warpgroups (64 accumulators) keep 96.  128 x 40 + 256 x 96 + 256 x 120
+// <= 640 x 96.
+constexpr int GEMM_REGS_PRODUCER = 40;
+constexpr int GEMM_REGS_EPILOGUE = 120;
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+// named barrier of the 256 MMA threads (id 1; id 0 is __syncthreads)
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // wgmma shared-memory descriptor: 128-byte swizzle, rows of 128 bytes, 8-row groups 1024 bytes apart
@@ -270,61 +326,73 @@ __device__ __forceinline__ void tile_epilogue(const GemmParams& p, const OutMaps
 }
 
 // ---- kernel ------------------------------------------------------------------------------------------
-template <int BN, int EPI, int STAGES>
-__global__ void __launch_bounds__(GEMM_THREADS, (gemm_ctas_per_sm<BN, EPI, STAGES>()))
+template <int BN, int EPI, int STAGES, bool PERSISTENT>
+__global__ void __launch_bounds__((gemm_threads<PERSISTENT>()), (gemm_ctas_per_sm<BN, EPI, STAGES, PERSISTENT>()))
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p,
                const __grid_constant__ OutMaps om) {
   static_assert(BN == 64 || BN == 128, "wgmma tiles: N = 64 or 128");
+  static_assert(gemm_smem_bytes<BN, EPI, STAGES, PERSISTENT>() <= 227 * 1024, "GEMM: shared memory");
   extern __shared__ uint8_t smem_raw[];
   constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
   constexpr int B_BYTES = BN * BLOCK_K * 2;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int W = BN / 2;
+  static_assert(!PERSISTENT || persistent_epilogue<EPI>(), "this epilogue runs one tile per CTA");
+  constexpr bool ONE_TILE = !PERSISTENT;
+  constexpr int WARP_TMA = gemm_warp_tma<PERSISTENT>();
 
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // swizzle-128B tiles need 1024-byte alignment
-  const uint32_t bar_base = base + region_bytes<BN, EPI, STAGES>();   // full[S], empty[S]; then 2 KB of row statistics
+  // full[S], empty[S], acc_full, acc_empty; then 2 KB of row statistics
+  const uint32_t bar_base = base + region_bytes<BN, EPI, STAGES, PERSISTENT>();
   const uint32_t full_bar0 = bar_base;
   const uint32_t empty_bar0 = bar_base + 8 * STAGES;
+  const uint32_t acc_full_bar = bar_base + 16 * STAGES;         // staging buffer holds a tile (256 MMA threads arrive)
+  const uint32_t acc_empty_bar = acc_full_bar + 8;              // the epilogue is done with it (256 epilogue threads)
   const uint32_t red_saddr = bar_base + 256;
   uint8_t* const gbase = smem_raw + (base - raw);
+  float* const acc = reinterpret_cast<float*>(gbase + acc_tile_offset<BN, EPI, STAGES, PERSISTENT>());
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int g = blockIdx.z;
-  const int m0 = blockIdx.x * BLOCK_M;
-  const int n0 = blockIdx.y * BN;
+  const int n_tiles_total = gemm_tile_count<BN>(p);
 
-  if (warp == GEMM_WARP_TMA && lane == 0) {
+  if (warp == WARP_TMA && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar0 + 8 * s, 1);
-      mbar_init(empty_bar0 + 8 * s, 8);            // one arrive per consumer warp
+      mbar_init(empty_bar0 + 8 * s, 8);            // one arrive per MMA warp
     }
+    mbar_init(acc_full_bar, 256);
+    mbar_init(acc_empty_bar, 256);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   pdl_wait();                    // everything above touched no global memory; operands of the previous kernel are now visible
 
-  if (warp == GEMM_WARP_TMA) {
-    // ===== TMA producer =====
-    if (elect_one()) {
+  if (warp >= WARP_TMA) {
+    // ===== TMA producer: the ring's stage and phase run on across tiles =====
+    if constexpr (!ONE_TILE) setmaxnreg_dec<GEMM_REGS_PRODUCER>();
+    if (warp == WARP_TMA && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      const int a_col0 = p.a_col_base + g * p.a_col_group_off;
-      const int a_row0 = m0 + g * p.a_row_group_off;
-      const int b_row0 = n0 + g * p.b_row_group_off;
-      for (int kc = 0; kc < p.k_chunks; ++kc) {
-        const int tap = kc / p.chunks_per_tap;
-        const int kin = kc - tap * p.chunks_per_tap;
-        mbar_wait(empty_bar0 + 8 * stage, phase ^ 1);
-        const uint32_t sa = base + stage * STAGE_BYTES;
-        const uint32_t fb = full_bar0 + 8 * stage;
-        mbar_expect_tx(fb, STAGE_BYTES);
-        tma_load_2d(sa, &tmA, fb, a_col0 + kin * BLOCK_K, a_row0 + p.tap_shift[tap]);
-        tma_load_2d(sa + A_BYTES, &tmB, fb, kc * BLOCK_K, b_row0);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x) {
+        const GemmTile tile = gemm_tile<BN>(p, t);
+        const int a_col0 = p.a_col_base + tile.g * p.a_col_group_off;
+        const int a_row0 = tile.m0 + tile.g * p.a_row_group_off;
+        const int b_row0 = tile.n0 + tile.g * p.b_row_group_off;
+        for (int kc = 0; kc < p.k_chunks; ++kc) {
+          const int tap = kc / p.chunks_per_tap;
+          const int kin = kc - tap * p.chunks_per_tap;
+          mbar_wait(empty_bar0 + 8 * stage, phase ^ 1);
+          const uint32_t sa = base + stage * STAGE_BYTES;
+          const uint32_t fb = full_bar0 + 8 * stage;
+          mbar_expect_tx(fb, STAGE_BYTES);
+          tma_load_2d(sa, &tmA, fb, a_col0 + kin * BLOCK_K, a_row0 + p.tap_shift[tap]);
+          tma_load_2d(sa + A_BYTES, &tmB, fb, kc * BLOCK_K, b_row0);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
       }
     }
     __syncwarp();
@@ -334,57 +402,82 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     return;
   }
 
-  // ===== consumers: warpgroup wg computes tile rows 64 wg .. 64 wg + 63 =====
-  const int wg = warp >> 2;
-  float d[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
-  {
+  if (warp < GEMM_WARP_EPI) {
+    // ===== MMA warpgroup wg computes tile rows 64 wg .. 64 wg + 63 =====
+    const int wg = warp >> 2;
     int stage = 0;
-    uint32_t phase = 0;
-    for (int kc = 0; kc < p.k_chunks; ++kc) {
-      mbar_wait(full_bar0 + 8 * stage, phase);
-      const uint32_t sa = base + stage * STAGE_BYTES;
-      const uint64_t da = gmma_desc_sw128(sa + wg * (64 * 128));
-      const uint64_t db = gmma_desc_sw128(sa + A_BYTES);
-      wgmma_fence();
+    uint32_t phase = 0, acc_phase = 0;
+    for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x) {
+      float d[BN / 2];
 #pragma unroll
-      for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)
-        // advance 32 bytes (16 fp16) along K inside the 128-byte swizzle row: +2 in the (addr>>4) field
-        wgmma_tile<BN>(d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), 1u);
-      wgmma_commit();
-      wgmma_wait<1>();                               // the previous chunk's MMAs have retired: release its stage
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      for (int kc = 0; kc < p.k_chunks; ++kc) {
+        mbar_wait(full_bar0 + 8 * stage, phase);
+        const uint32_t sa = base + stage * STAGE_BYTES;
+        const uint64_t da = gmma_desc_sw128(sa + wg * (64 * 128));
+        const uint64_t db = gmma_desc_sw128(sa + A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)
+          // advance 32 bytes (16 fp16) along K inside the 128-byte swizzle row: +2 in the (addr>>4) field
+          wgmma_tile<BN>(d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), 1u);
+        wgmma_commit();
+        wgmma_wait<1>();                               // the previous chunk's MMAs have retired: release its stage
+        reg_fence(d);
+        if (kc > 0 && lane == 0) mbar_arrive(empty_bar0 + 8 * (stage == 0 ? STAGES - 1 : stage - 1));
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
       reg_fence(d);
-      if (kc > 0 && lane == 0) mbar_arrive(empty_bar0 + 8 * (stage == 0 ? STAGES - 1 : stage - 1));
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    reg_fence(d);
-  }
-  pdl_trigger();                 // main loop done: the next kernel's CTAs may start their prologue under our epilogue
+      if (lane == 0) mbar_arrive(empty_bar0 + 8 * (stage == 0 ? STAGES - 1 : stage - 1));
+      if (t + (int)gridDim.x >= n_tiles_total) pdl_trigger();   // last K loop done: the next kernel may start its prologue
 
-  // ===== park the accumulators in the (now idle) ring, then the epilogue by all 8 consumer warps =====
-  consumer_sync();               // both warpgroups have finished reading the ring
-  float* acc = reinterpret_cast<float*>(gbase + acc_tile_offset<BN, EPI>());
-  {
-    // fragment layout of wgmma m64nNk16: d[4j + 2h + e] = (row 16 (warp & 3) + lane / 4 + 8 h, column 8 j + 2 (lane & 3) + e)
-    const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      // ===== hand the accumulators to the epilogue through the staging buffer =====
+      if constexpr (ONE_TILE) consumer_sync();      // the staging buffer is the ring: both warpgroups are done reading it
+      else mbar_wait(acc_empty_bar, acc_phase ^ 1);
+      // fragment layout of wgmma m64nNk16: d[4j + 2h + e] = (row 16 (warp & 3) + lane / 4 + 8 h, column 8 j + 2 (lane & 3) + e)
+      const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
+      for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = r_base + 8 * h, c = 8 * j + 2 * (lane & 3);
-        float* dst = acc + ((r >> 5) + 4 * (c / W)) * acc_block_floats<BN>() + (r & 31) * (W + 4) + (c % W);
-        *reinterpret_cast<float2*>(dst) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+        for (int h = 0; h < 2; ++h) {
+          const int r = r_base + 8 * h, c = 8 * j + 2 * (lane & 3);
+          float* dst = acc + ((r >> 5) + 4 * (c / W)) * acc_block_floats<BN>() + (r & 31) * (W + 4) + (c % W);
+          *reinterpret_cast<float2*>(dst) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+        }
+      }
+      if constexpr (ONE_TILE) {
+        consumer_sync();
+        const GemmTile tile = gemm_tile<BN>(p, t);
+        tile_epilogue<BN, EPI>(p, om, tile.g, tile.m0, tile.n0, tile.n_tile, warp & 3, warp >> 2, lane, acc,
+                               reinterpret_cast<float*>(smem_raw + (red_saddr - raw)), red_saddr,
+                               reinterpret_cast<float*>(gbase + warp * DUAL_STAGE_BYTES),
+                               reinterpret_cast<float*>(gbase + 8 * DUAL_STAGE_BYTES) + warp * 64);
+      } else {
+        mbar_arrive(acc_full_bar);
+        acc_phase ^= 1;
       }
     }
+    if constexpr (EPI == EPI_DUAL) { if (p.out_tma && lane == 0) tma_store_wait_all(); }   // smem must outlive the bulk reads
+    return;
   }
-  consumer_sync();
-  tile_epilogue<BN, EPI>(p, om, g, m0, n0, (int)blockIdx.y, warp & 3, warp >> 2, lane, acc,
-                         reinterpret_cast<float*>(smem_raw + (red_saddr - raw)), red_saddr,
-                         reinterpret_cast<float*>(gbase + warp * DUAL_STAGE_BYTES),
-                         reinterpret_cast<float*>(gbase + 8 * DUAL_STAGE_BYTES) + warp * 64);
-  if constexpr (EPI == EPI_DUAL) { if (p.out_tma && lane == 0) tma_store_wait_all(); }   // smem must outlive the bulk reads
+
+  // ===== epilogue warps (persistent instantiations only) =====
+  if constexpr (ONE_TILE) return;
+  setmaxnreg_inc<GEMM_REGS_EPILOGUE>();
+  const int ew = warp - GEMM_WARP_EPI;
+  uint32_t acc_phase = 0;
+  for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x) {
+    const GemmTile tile = gemm_tile<BN>(p, t);
+    mbar_wait(acc_full_bar, acc_phase);
+    if (t + (int)gridDim.x >= n_tiles_total) pdl_trigger();
+    tile_epilogue<BN, EPI>(p, om, tile.g, tile.m0, tile.n0, tile.n_tile, ew & 3, ew >> 2, lane, acc,
+                           reinterpret_cast<float*>(smem_raw + (red_saddr - raw)), red_saddr,
+                           reinterpret_cast<float*>(gbase + ew * DUAL_STAGE_BYTES),
+                           reinterpret_cast<float*>(gbase + 8 * DUAL_STAGE_BYTES) + ew * 64);
+    mbar_arrive(acc_empty_bar);
+    acc_phase ^= 1;
+  }
 }
 
 }  // namespace mk

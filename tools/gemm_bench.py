@@ -1,5 +1,11 @@
 """Device times of the ViT-B GEMMs at the C3 batch (64 images = 124096 tokens) and of the head convolution, for A/B runs of
-GEMM changes:   python tools/gemm_bench.py [n_images]"""
+GEMM changes:   python tools/gemm_bench.py [n_images]
+
+Next to each ViT GEMM's rate it prints the HBM bytes of two traffic models and the bandwidth they imply at the measured
+time.  "m-fastest" is a tile order that walks the M-tiles fastest: A (far larger than the L2) is evicted before the grid
+reaches the next column of N-tiles, so it is read once per column.  "n-fastest" is gemm_tile()'s order: every A
+row-panel is read once while all of B stays in L2.  Both count B once, the output once and the fp32 residual of RESID_F
+twice (read and write).  The bytes are computed from the shapes, not measured."""
 import os
 import sys
 
@@ -47,7 +53,10 @@ for name, N_, K_, epi, kw in (
         ("fc2", D, 4 * D, "RESID_F", dict(bias=torch.randn(D, device=dev), gamma=g, out_f=x32, out_f_ld=D))):
     us = timeit(lin(N_, K_, epi, **kw))
     total += us
-    print(f"{tag} vit-b.{name:9s} {M}x{N_}x{K_}: {us:9.1f} us  {2 * M * N_ * K_ / us / 1e6:7.1f} TFLOP/s", flush=True)
+    a_bytes, rest = M * K_ * 2, N_ * K_ * 2 + (M * N_ * 2 if epi == "STORE_H" else 2 * M * N_ * 4)
+    traffic = {"m-fastest": a_bytes * (N_ // 128) + rest, "n-fastest": a_bytes + rest}
+    model = "  ".join(f"{k} {b / 1e9:5.2f} GB = {b / us / 1e3:5.0f} GB/s" for k, b in traffic.items())
+    print(f"{tag} vit-b.{name:9s} {M}x{N_}x{K_}: {us:9.1f} us  {2 * M * N_ * K_ / us / 1e6:7.1f} TFLOP/s  {model}", flush=True)
     del kw
 print(f"{tag} vit-b block GEMMs: {total:9.1f} us", flush=True)
 big = 16384
