@@ -33,12 +33,16 @@ static PFN_encodeTiled get_encode() {
 // weight buffers every call, so they are cached.
 struct MapKey {
   const void* ptr; long long rows, cols, ld; int box;
-  bool operator==(const MapKey& o) const { return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box == o.box; }
+  long long groups;          // 0: 2-D operand map; > 0: 3-D output map over [groups, rows, cols]
+  bool operator==(const MapKey& o) const {
+    return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box == o.box && groups == o.groups;
+  }
 };
 struct MapKeyHash {
   size_t operator()(const MapKey& k) const {
     size_t h = reinterpret_cast<size_t>(k.ptr);
     h = h * 1000003u ^ (size_t)k.rows; h = h * 1000003u ^ (size_t)k.cols; h = h * 1000003u ^ (size_t)k.ld;
+    h = h * 1000003u ^ (size_t)k.groups;
     return h * 1000003u ^ (size_t)k.box;
   }
 };
@@ -47,19 +51,29 @@ static std::mutex g_map_mutex;
 
 static int encode_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems,
                                  int box_rows);
+static int encode_tensor_map_out_f16(CUtensorMap* map, const void* ptr, long long groups, long long rows, long long cols,
+                                     int box_rows);
 
-int make_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems,
-                        int box_rows) {
-  MapKey key{ptr, rows, cols, ld_elems, box_rows};
+static int cached_map(const MapKey& key, CUtensorMap* map) {
   std::lock_guard<std::mutex> lock(g_map_mutex);
   auto it = g_map_cache.find(key);
   if (it != g_map_cache.end()) { *map = it->second; return MK_OK; }
-  int rc = encode_tensor_map_f16(map, ptr, rows, cols, ld_elems, box_rows);
+  int rc = key.groups ? encode_tensor_map_out_f16(map, key.ptr, key.groups, key.rows, key.cols, key.box)
+                      : encode_tensor_map_f16(map, key.ptr, key.rows, key.cols, key.ld, key.box);
   if (rc == MK_OK) {
     if (g_map_cache.size() > 4096) g_map_cache.clear();
     g_map_cache.emplace(key, *map);
   }
   return rc;
+}
+
+int make_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems,
+                        int box_rows) {
+  return cached_map(MapKey{ptr, rows, cols, ld_elems, box_rows, 0}, map);
+}
+
+int make_tensor_map_out_f16(CUtensorMap* map, void* ptr, long long groups, long long rows, long long cols, int box_rows) {
+  return cached_map(MapKey{ptr, rows, cols, cols, box_rows, groups}, map);
 }
 
 static int encode_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems,
@@ -78,6 +92,27 @@ static int encode_tensor_map_f16(CUtensorMap* map, const void* ptr, long long ro
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_last_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return MK_ERR_CUDA; }
+  return MK_OK;
+}
+
+// Contiguous fp16 [groups][rows][cols] output: box = 64 columns (128 bytes) x box_rows rows x 1, 128-byte swizzle on the
+// shared-memory side, rows beyond `rows` clipped by the hardware in every group.
+static int encode_tensor_map_out_f16(CUtensorMap* map, const void* ptr, long long groups, long long rows, long long cols,
+                                     int box_rows) {
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) { set_last_error("cuTensorMapEncodeTiled entry point not available"); return MK_ERR_CUDA; }
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (cols % 8)) {
+    set_last_error("TMA output must be 16-byte aligned with cols %% 8 == 0 (ptr=%p cols=%lld)", ptr, cols);
+    return MK_ERR_INVALID;
+  }
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)groups};
+  cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)cols * 2 * (cuuint64_t)rows};
+  cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_last_error("cuTensorMapEncodeTiled (fp16 output) failed with CUresult %d", (int)r); return MK_ERR_CUDA; }
   return MK_OK;
 }
 
@@ -187,7 +222,7 @@ static bool use_simt() {
   return v == 1;
 }
 
-static int sm_count() {
+int sm_count() {
   static int n[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);

@@ -12,6 +12,9 @@ struct GemmOperand {       // a row-major fp16 matrix [rows, cols] with leading 
 enum GemmImpl : int { GEMM_IMPL_DEFAULT = 0, GEMM_IMPL_TC = 1, GEMM_IMPL_SIMT = 2 };
 
 int make_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems, int box_rows);
+// TMA store map of a contiguous fp16 [groups, rows, cols] tensor (box 64 columns x box_rows rows, 128-byte swizzle)
+int make_tensor_map_out_f16(CUtensorMap* map, void* ptr, long long groups, long long rows, long long cols, int box_rows);
+int sm_count();            // SMs of the current device
 int launch_gemm(int epi, const GemmOperand& A, const GemmOperand& B, const GemmParams& p, cudaStream_t stream,
                 int impl = GEMM_IMPL_DEFAULT);
 // true when launch_gemm would put a [M, N] x (64 k_chunks) residual GEMM on a one-tile kernel, i.e. EPI_RESID_LN may be used
