@@ -56,6 +56,9 @@ int mk_set_tensor(mk_handle* h, const char* name, const void* ptr_dev, int dtype
 int mk_finalize(mk_handle* h, int img_h, int img_w);
 
 long long mk_workspace_bytes(mk_handle* h, int n_pairs, int img_h, int img_w);
+/* Workspace of a call that extracts n_img images and matches / solves n_pairs pairs: (n, 0) for mk_extract_images,
+ * (0, P) for mk_forward_pairs; (2P, P) equals mk_workspace_bytes(P). */
+long long mk_workspace_bytes_for(mk_handle* h, int n_img, int n_pairs, int img_h, int img_w);
 /* Byte offset of a named intermediate buffer inside the workspace (debugging / stage-wise tests; names and
  * layouts are listed in DESIGN.md §3: "X", "F", "CAT", "Y4d", ...). */
 long long mk_workspace_offset(mk_handle* h, const char* name, int n_pairs, int img_h, int img_w);
@@ -74,6 +77,16 @@ int mk_extract(mk_handle* h, const float* images_dev, int n_pairs, int img_h, in
  * bit-identical to mk_extract on the reference's float tensor. */
 int mk_extract_u8(mk_handle* h, const unsigned char* images_u8_dev, int n_pairs, int img_h, int img_w, float* kps_dev,
                   float* depth_dev, float* scr_dev, float* dsc_dev, void* ws_dev, long long ws_bytes, void* stream);
+
+/* Stage 1 for any number of images (n_img >= 1, odd counts included), e.g. a feature bank for mk_forward_pairs: one
+ * Map-free reference image and its queries are extracted once each instead of once per pair.  images_dev fp32
+ * [n_img, 3, H, W] / images_u8_dev uint8 [n_img, H, W, 3]; kps [n_img,2,N], depth [n_img,1,N], scr [n_img,1,N],
+ * dsc [n_img,128,N], bit-identical to what mk_extract writes for the same image.  Workspace:
+ * mk_workspace_bytes_for(n_img, 0).  The matcher operands this leaves in the workspace are not meant for mk_match. */
+int mk_extract_images(mk_handle* h, const float* images_dev, int n_img, int img_h, int img_w, float* kps_dev,
+                      float* depth_dev, float* scr_dev, float* dsc_dev, void* ws_dev, long long ws_bytes, void* stream);
+int mk_extract_images_u8(mk_handle* h, const unsigned char* images_u8_dev, int n_img, int img_h, int img_w, float* kps_dev,
+                         float* depth_dev, float* scr_dev, float* dsc_dev, void* ws_dev, long long ws_bytes, void* stream);
 
 /* ---- stage 2: dual-softmax matcher
  * replaces featureMatcher/dualSoftmax.forward (feature_matcher.py:48-83), kp_matrix_scores
@@ -121,6 +134,24 @@ int mk_forward_u8(mk_handle* h, const unsigned char* images_u8_dev, const float*
                   float* dsc_dev, float* scores_dev, float* kp_scores_dev, float* final_scores_dev, long long nn_pitch,
                   float* pose_dev, int* best_set_dev, float* inlier_mask_dev, int* sampled_idx_out_dev, int* status_dev,
                   void* ws_dev, long long ws_bytes, void* stream);
+
+/* ---- stages 2 + 3 on pairs drawn from feature banks: replaces MickeyRelativePose.forward (compute_pose.py:20-37) for
+ * pairs (bank0[idx0[p]], bank1[idx1[p]]) whose features mk_extract_images already computed.
+ * bank b: kps [n_b,2,N], depth [n_b,1,N], scr [n_b,1,N], dsc [n_b,128,N] as mk_extract_images writes them, extracted at
+ * the finalized geometry (so N x N stays square); bank0 and bank1 may be the same tensors.  idx0_dev / idx1_dev int32
+ * [n_pairs] (device).  One gather kernel builds the matcher's role-0 / role-1 descriptor operands (the hi/lo fp16
+ * split of mk_extract) and the solver's pair-major operands; the matcher and the solver then run as in mk_forward, so
+ * the outputs are bit-identical to mk_forward on the same images with the same seed.
+ * Out: kps_dev [2*n_pairs,2,N], depth_dev [2*n_pairs,1,N] (required: the solver reads them; role-0 rows first), and
+ * scores / kp_scores / final_scores / nn_pitch / pose / best_set / inlier_mask / sampled_idx as in mk_forward.
+ * status_dev bit3 = an index outside [0, n_b): nothing outside a bank is read, and the batch gets the zero pose of the
+ * other status bits (R = 0, t = 0, inliers = 0).  Workspace: mk_workspace_bytes_for(0, n_pairs). */
+int mk_forward_pairs(mk_handle* h, const float* kps0_dev, const float* depth0_dev, const float* scr0_dev, const float* dsc0_dev,
+                     int n0, const float* kps1_dev, const float* depth1_dev, const float* scr1_dev, const float* dsc1_dev, int n1,
+                     const int* idx0_dev, const int* idx1_dev, const float* K0_dev, const float* K1_dev, int n_pairs,
+                     unsigned long long seed, float* kps_dev, float* depth_dev, float* scores_dev, float* kp_scores_dev,
+                     float* final_scores_dev, long long nn_pitch, float* pose_dev, int* best_set_dev, float* inlier_mask_dev,
+                     int* sampled_idx_out_dev, int* status_dev, void* ws_dev, long long ws_bytes, void* stream);
 
 /* ---- after the path: submission records (replaces the per-pair loop of submission.py:43-59)
  * pose_dev fp32 [n_pairs,13] as written by mk_forward / mk_solve_pose -> out_dev fp64 [n_pairs, 9] =

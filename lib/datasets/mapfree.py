@@ -9,7 +9,9 @@ On-disk format (one directory per scene under <DATA_ROOT>/<split>/):
 val / test pairs = (seq0 frame 0, every SAMPLE_FACTOR-th seq1 frame of poses.txt)       (mapfree.py:94-103)
 
 `uint8_images=True` returns the images as uint8 [h, w, 3] (what cv2 hands over) for the fused ingest kernel
-(mk_forward_u8); the default returns the reference's float [3, h, w] tensors.
+(mk_forward_u8); the default returns the reference's float [3, h, w] tensors.  `skip_image0=True` leaves `image0` out of
+every item: a caller that extracts each scene's reference image once (tools/run_submission.py --share-reference) reads
+it itself, once per scene, instead of the loader decoding it once per pair.
 """
 from pathlib import Path
 
@@ -35,7 +37,7 @@ def _rows(path: Path):
 
 class MapFreeScene(data.Dataset):
     def __init__(self, scene_root, resize, sample_factor=1, overlap_limits=None, transforms=None, test_scene=False,
-                 uint8_images=False):
+                 uint8_images=False, skip_image0=False):
         super().__init__()
         self.scene_root = Path(scene_root)
         self.resize = resize
@@ -43,6 +45,7 @@ class MapFreeScene(data.Dataset):
         self.transforms = transforms
         self.test_scene = test_scene
         self.uint8_images = uint8_images
+        self.skip_image0 = skip_image0
         self.poses = self.read_poses(self.scene_root)
         self.K, self.K_ori = self.read_intrinsics(self.scene_root, resize)
         self.pairs = self.load_pairs(self.scene_root, overlap_limits, sample_factor)
@@ -89,7 +92,8 @@ class MapFreeScene(data.Dataset):
         return len(self.pairs)
 
     # ---- one pair ----------------------------------------------------------------------------------------------
-    def _image(self, rel):
+    def image(self, rel):
+        """One image of the scene as the items carry it (resized; uint8 HWC or float CHW)."""
         u8 = read_color_image_u8(self.scene_root / rel, self.resize)
         if self.uint8_images:
             return u8
@@ -113,19 +117,21 @@ class MapFreeScene(data.Dataset):
             (qA, cA), (qB, cB) = (np.zeros([4]), np.zeros([3])), (np.zeros([4]), np.zeros([3]))
         else:
             T, (qA, cA), (qB, cB) = self.relative_pose(nameA, nameB)
-        return {
-            "image0": self._image(nameA), "image1": self._image(nameB),
+        item = {} if self.skip_image0 else {"image0": self.image(nameA)}
+        item.update({
+            "image1": self.image(nameB),
             "T_0to1": torch.from_numpy(T),
             "abs_q_0": qA, "abs_c_0": cA, "abs_q_1": qB, "abs_c_1": cB,
             "K_color0": self.K[nameA], "Kori_color0": self.K_ori[nameA],
             "K_color1": self.K[nameB], "Kori_color1": self.K_ori[nameB],
             "dataset_name": "Mapfree", "scene_id": self.scene_root.stem, "scene_root": str(self.scene_root),
             "pair_id": index * self.sample_factor, "pair_names": (nameA, nameB),
-        }
+        })
+        return item
 
 
 class MapFreeDataset(data.ConcatDataset):
-    def __init__(self, cfg, mode, transforms=None, uint8_images=False):
+    def __init__(self, cfg, mode, transforms=None, uint8_images=False, skip_image0=False):
         assert mode in SAMPLE_FACTOR, "Invalid dataset mode"
         root = Path(cfg.DATASET.DATA_ROOT) / mode
         scenes = cfg.DATASET.SCENES
@@ -135,5 +141,6 @@ class MapFreeDataset(data.ConcatDataset):
             scenes = scenes[:30] if mode == "train" else scenes[:10] if mode == "val" else scenes
         window = (cfg.DATASET.MIN_OVERLAP_SCORE, cfg.DATASET.MAX_OVERLAP_SCORE)
         size = (cfg.DATASET.WIDTH, cfg.DATASET.HEIGHT)
-        super().__init__([MapFreeScene(root / s, size, SAMPLE_FACTOR[mode], window, transforms, mode == "test", uint8_images)
+        super().__init__([MapFreeScene(root / s, size, SAMPLE_FACTOR[mode], window, transforms, mode == "test", uint8_images,
+                                       skip_image0)
                           for s in scenes])

@@ -71,6 +71,17 @@ EXPORTS = {
                              C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
     "mk_extract_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_workspace_bytes_for": (C.c_longlong, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_extract_images": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_extract_images_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_forward_pairs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_ulonglong,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,
+                                   C.c_void_p]),
     "mk_match": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p]),
     "mk_solve_pose": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                 C.c_ulonglong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -4,6 +4,7 @@
 #include "gemm.h"
 #include "ops.h"
 
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <unordered_map>
@@ -29,16 +30,18 @@ struct mk_handle {
 
 namespace {
 
+// n_img: images one call extracts; n_pairs: pairs it matches and solves.  mk_forward and its stages: (2P, P);
+// mk_extract_images: (n, 0); mk_forward_pairs: (0, P).
 struct Geo {
-  int H, W, gh, gw, N, T, h2, w2, per_img, n_img;
+  int H, W, gh, gw, N, T, h2, w2, per_img, n_img, n_pairs;
   long long M, Mp, R;
 };
 
-Geo make_geo(int n_pairs, int H, int W) {
+Geo make_geo(int n_img, int n_pairs, int H, int W) {
   Geo g;
   g.H = H; g.W = W; g.gh = H / 14; g.gw = W / 14;
   g.N = g.gh * g.gw; g.T = g.N + 1; g.h2 = g.gh + 2; g.w2 = g.gw + 2; g.per_img = g.h2 * g.w2;
-  g.n_img = 2 * n_pairs;
+  g.n_img = n_img; g.n_pairs = n_pairs;
   g.M = (long long)g.n_img * g.T; g.Mp = (long long)g.n_img * g.N; g.R = (long long)g.n_img * g.per_img;
   return g;
 }
@@ -73,10 +76,13 @@ struct Workspace {
   size_t bytes;
 };
 
-Workspace carve(void* base, const mk_config& c, const Geo& g, int n_pairs) {
+Workspace carve(void* base, const mk_config& c, const Geo& g) {
   Workspace w;
   Carver cv(base);
+  const int n_pairs = g.n_pairs;
   const size_t D = c.embed_dim, M = g.M, R = g.R;
+  // the matcher's operands: written by the extraction (n_img images) or by the bank gather (2 * n_pairs role rows)
+  const size_t n_op = (size_t)std::max(g.n_img, 2 * g.n_pairs);
   const int* bd = c.block_dims;
   w.P = cv.take<__half>((size_t)g.Mp * KPAD);
   w.X = cv.take<float>(M * D);
@@ -95,9 +101,9 @@ Workspace carve(void* base, const mk_config& c, const Geo& g, int n_pairs) {
   w.KVP = cv.take<float>((size_t)g.n_img * G * linattn_kv_chunks(g.h2, g.w2) * 8 * 272);
   w.Y4k = cv.take<float>(R * 3 * bd[3]); w.Y4d = cv.take<float>(R * c.desc_dim);
   w.score_raw = cv.take<float>((size_t)g.n_img * g.N);
-  w.DSCX = cv.take<__half>((size_t)g.n_img * g.N * 384);
+  w.DSCX = cv.take<__half>(n_op * g.N * 384);
   w.nrm2 = cv.take<float>((size_t)g.n_img * g.N);
-  w.scr_copy = cv.take<float>((size_t)g.n_img * g.N);
+  w.scr_copy = cv.take<float>(n_op * g.N);
   const size_t npad = (size_t)ceil_div(g.N, 128) * 128;          // matcher: float2 partials [pair][slot][npad], lse vectors [pair][npad]
   w.part_row = cv.take<float>((size_t)n_pairs * (npad / 64) * npad * 2); w.part_col = cv.take<float>((size_t)n_pairs * (npad / 32) * npad * 2);
   w.lse_r = cv.take<float>((size_t)n_pairs * npad); w.lse_c = cv.take<float>((size_t)n_pairs * npad);
@@ -175,10 +181,10 @@ int gemm(mk_handle* h, const char* tag, int epi, const void* a, long long a_rows
 
 // ---- stage 1 ----------------------------------------------------------------------------------------------
 // img_fmt 0: fp32 NCHW in [0,1] (the reference's tensors); 1: uint8 NHWC RGB as cv2 delivers it (mk_*_u8, SURVEY.md §8 f1)
-int run_extract(mk_handle* h, const void* images, int img_fmt, int n_pairs, int H, int W, float* kps, float* depth, float* scr,
+int run_extract(mk_handle* h, const void* images, int img_fmt, const Geo& g, float* kps, float* depth, float* scr,
                 float* dsc, Workspace& w, cudaStream_t st) {
   const mk_config& c = h->cfg;
-  const Geo g = make_geo(n_pairs, H, W);
+  const int H = g.H, W = g.W;
   const int D = c.embed_dim;
   Lookup L{h};
   // -- tokens: patch embedding + cls + position embedding (dinov2.py:191-200)
@@ -417,15 +423,15 @@ int run_solve(mk_handle* h, const float* final_scores, long long nn_pitch, const
   return MK_OK;
 }
 
-int check_ws(mk_handle* h, int n_pairs, int H, int W, void* ws, long long ws_bytes, Workspace& out) {
+int check_ws(mk_handle* h, int n_img, int n_pairs, int H, int W, void* ws, long long ws_bytes, Workspace& out) {
   if (!h || !h->finalized) { set_last_error("handle not finalized"); return MK_ERR_INVALID; }
   MK_CUDA_CHECK(cudaSetDevice(h->device));        // one handle per device: every entry point runs on the handle's device
   if (H != h->geo_h || W != h->geo_w) {
     set_last_error("geometry %dx%d does not match the finalized geometry %dx%d", H, W, h->geo_h, h->geo_w);
     return MK_ERR_INVALID;
   }
-  const Geo g = make_geo(n_pairs, H, W);
-  out = carve(ws, h->cfg, g, n_pairs);
+  const Geo g = make_geo(n_img, n_pairs, H, W);
+  out = carve(ws, h->cfg, g);
   if (!ws || (long long)out.bytes > ws_bytes) {
     set_last_error("workspace too small: need %zu bytes, got %lld", out.bytes, ws_bytes);
     return MK_ERR_INVALID;
@@ -495,29 +501,55 @@ int mk_finalize(mk_handle* h, int H, int W) {
 
 long long mk_workspace_bytes(mk_handle* h, int n_pairs, int H, int W) {
   if (!h) return -1;
-  const Geo g = make_geo(n_pairs, H, W);
-  return (long long)carve(nullptr, h->cfg, g, n_pairs).bytes;
+  return (long long)carve(nullptr, h->cfg, make_geo(2 * n_pairs, n_pairs, H, W)).bytes;
+}
+
+long long mk_workspace_bytes_for(mk_handle* h, int n_img, int n_pairs, int H, int W) {
+  if (!h || n_img < 0 || n_pairs < 0) return -1;
+  const Geo g = make_geo(n_img, n_pairs, H, W);
+  return (long long)carve(nullptr, h->cfg, g).bytes;
 }
 
 int mk_extract(mk_handle* h, const float* images, int n_pairs, int H, int W, float* kps, float* depth, float* scr,
                float* dsc, void* ws, long long ws_bytes, void* stream) {
   Workspace w;
-  MK_TRY(check_ws(h, n_pairs, H, W, ws, ws_bytes, w));
-  return run_extract(h, images, 0, n_pairs, H, W, kps, depth, scr, dsc, w, (cudaStream_t)stream);
+  MK_TRY(check_ws(h, 2 * n_pairs, n_pairs, H, W, ws, ws_bytes, w));
+  return run_extract(h, images, 0, make_geo(2 * n_pairs, n_pairs, H, W), kps, depth, scr, dsc, w, (cudaStream_t)stream);
 }
 
 int mk_extract_u8(mk_handle* h, const unsigned char* images, int n_pairs, int H, int W, float* kps, float* depth, float* scr,
                   float* dsc, void* ws, long long ws_bytes, void* stream) {
   Workspace w;
-  MK_TRY(check_ws(h, n_pairs, H, W, ws, ws_bytes, w));
-  return run_extract(h, images, 1, n_pairs, H, W, kps, depth, scr, dsc, w, (cudaStream_t)stream);
+  MK_TRY(check_ws(h, 2 * n_pairs, n_pairs, H, W, ws, ws_bytes, w));
+  return run_extract(h, images, 1, make_geo(2 * n_pairs, n_pairs, H, W), kps, depth, scr, dsc, w, (cudaStream_t)stream);
+}
+
+static int extract_images_any(mk_handle* h, const void* images, int img_fmt, int n_img, int H, int W, float* kps, float* depth,
+                              float* scr, float* dsc, void* ws, long long ws_bytes, void* stream) {
+  if (n_img <= 0 || !images || !kps || !depth || !scr || !dsc) {
+    set_last_error("mk_extract_images: n_img %d must be positive and every pointer non-NULL", n_img);
+    return MK_ERR_INVALID;
+  }
+  Workspace w;
+  MK_TRY(check_ws(h, n_img, 0, H, W, ws, ws_bytes, w));
+  return run_extract(h, images, img_fmt, make_geo(n_img, 0, H, W), kps, depth, scr, dsc, w, (cudaStream_t)stream);
+}
+
+int mk_extract_images(mk_handle* h, const float* images, int n_img, int H, int W, float* kps, float* depth, float* scr,
+                      float* dsc, void* ws, long long ws_bytes, void* stream) {
+  return extract_images_any(h, images, 0, n_img, H, W, kps, depth, scr, dsc, ws, ws_bytes, stream);
+}
+
+int mk_extract_images_u8(mk_handle* h, const unsigned char* images, int n_img, int H, int W, float* kps, float* depth, float* scr,
+                         float* dsc, void* ws, long long ws_bytes, void* stream) {
+  return extract_images_any(h, images, 1, n_img, H, W, kps, depth, scr, dsc, ws, ws_bytes, stream);
 }
 
 int mk_match(mk_handle* h, int n_pairs, float* scores, float* kp_scores, float* final_scores, long long nn_pitch, void* ws,
              long long ws_bytes, void* stream) {
   Workspace w;
-  MK_TRY(check_ws(h, n_pairs, h ? h->geo_h : 0, h ? h->geo_w : 0, ws, ws_bytes, w));
-  const Geo g = make_geo(n_pairs, h->geo_h, h->geo_w);
+  MK_TRY(check_ws(h, 2 * n_pairs, n_pairs, h ? h->geo_h : 0, h ? h->geo_w : 0, ws, ws_bytes, w));
+  const Geo g = make_geo(2 * n_pairs, n_pairs, h->geo_h, h->geo_w);
   return run_match(h, n_pairs, g.N, scores, kp_scores, final_scores, nn_pitch, w, (cudaStream_t)stream);
 }
 
@@ -526,8 +558,8 @@ int mk_solve_pose(mk_handle* h, const float* final_scores, long long nn_pitch, c
                   const int* inner_idx, float* pose, int* best_set, float* inl_mask, int* sampled_out,
                   float* hyp_scores_out, int* status, void* ws, long long ws_bytes, void* stream) {
   Workspace w;
-  MK_TRY(check_ws(h, n_pairs, h ? h->geo_h : 0, h ? h->geo_w : 0, ws, ws_bytes, w));
-  const Geo g = make_geo(n_pairs, h->geo_h, h->geo_w);
+  MK_TRY(check_ws(h, 2 * n_pairs, n_pairs, h ? h->geo_h : 0, h ? h->geo_w : 0, ws, ws_bytes, w));
+  const Geo g = make_geo(2 * n_pairs, n_pairs, h->geo_h, h->geo_w);
   if (n_kpts != g.N) { set_last_error("n_kpts %d does not match the geometry (%d)", n_kpts, g.N); return MK_ERR_INVALID; }
   return run_solve(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, n_kpts, seed, outer_idx, inner_idx, pose, best_set,
                    inl_mask, sampled_out, hyp_scores_out, status, w, (cudaStream_t)stream);
@@ -538,10 +570,10 @@ static int forward_any(mk_handle* h, const void* images, int img_fmt, const floa
                        float* kp_scores, float* final_scores, long long nn_pitch, float* pose, int* best_set, float* inl_mask,
                        int* sampled_out, int* status, void* ws, long long ws_bytes, void* stream) {
   Workspace w;
-  MK_TRY(check_ws(h, n_pairs, H, W, ws, ws_bytes, w));
-  const Geo g = make_geo(n_pairs, H, W);
+  MK_TRY(check_ws(h, 2 * n_pairs, n_pairs, H, W, ws, ws_bytes, w));
+  const Geo g = make_geo(2 * n_pairs, n_pairs, H, W);
   cudaStream_t st = (cudaStream_t)stream;
-  MK_TRY(run_extract(h, images, img_fmt, n_pairs, H, W, kps, depth, scr, dsc, w, st));
+  MK_TRY(run_extract(h, images, img_fmt, g, kps, depth, scr, dsc, w, st));
   MK_TRY(run_match(h, n_pairs, g.N, scores, kp_scores, final_scores, nn_pitch, w, st));
   return run_solve(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, g.N, seed, nullptr, nullptr, pose, best_set, inl_mask,
                    sampled_out, nullptr, status, w, st);
@@ -563,6 +595,30 @@ int mk_forward_u8(mk_handle* h, const unsigned char* images, const float* K0, co
                      pose, best_set, inl_mask, sampled_out, status, ws, ws_bytes, stream);
 }
 
+int mk_forward_pairs(mk_handle* h, const float* kps0, const float* depth0, const float* scr0, const float* dsc0, int n0,
+                     const float* kps1, const float* depth1, const float* scr1, const float* dsc1, int n1, const int* idx0,
+                     const int* idx1, const float* K0, const float* K1, int n_pairs, unsigned long long seed, float* kps, float* depth,
+                     float* scores, float* kp_scores, float* final_scores, long long nn_pitch, float* pose, int* best_set,
+                     float* inl_mask, int* sampled_out, int* status, void* ws, long long ws_bytes, void* stream) {
+  if (n_pairs <= 0 || n0 <= 0 || n1 <= 0 || !kps0 || !depth0 || !scr0 || !dsc0 || !kps1 || !depth1 || !scr1 || !dsc1 || !idx0 ||
+      !idx1 || !K0 || !K1 || !kps || !depth || !pose) {
+    set_last_error("mk_forward_pairs: n_pairs %d, bank sizes %d / %d must be positive; banks, indices, K, kps, depth and pose "
+                   "must be non-NULL", n_pairs, n0, n1);
+    return MK_ERR_INVALID;
+  }
+  Workspace w;
+  MK_TRY(check_ws(h, 0, n_pairs, h ? h->geo_h : 0, h ? h->geo_w : 0, ws, ws_bytes, w));
+  const Geo g = make_geo(0, n_pairs, h->geo_h, h->geo_w);
+  cudaStream_t st = (cudaStream_t)stream;
+  const BankView b0{kps0, depth0, scr0, dsc0, idx0, n0}, b1{kps1, depth1, scr1, dsc1, idx1, n1};
+  MK_KERNEL("pairs.gather", bank_gather(b0, b1, n_pairs, g.N, w.DSCX, kps, depth, w.scr_copy, st));
+  MK_TRY(run_match(h, n_pairs, g.N, scores, kp_scores, final_scores, nn_pitch, w, st));
+  MK_TRY(run_solve(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, g.N, seed, nullptr, nullptr, pose, best_set, inl_mask,
+                   sampled_out, nullptr, status, w, st));
+  MK_KERNEL("pairs.index_check", bank_index_check(b0, b1, n_pairs, pose, status, st));
+  return MK_OK;
+}
+
 int mk_pose_to_submission(const float* pose, int n_pairs, double* out, void* stream) {
   if (!pose || !out || n_pairs < 0) { set_last_error("null argument"); return MK_ERR_INVALID; }
   return pose_to_submission(pose, n_pairs, out, (cudaStream_t)stream);
@@ -577,9 +633,9 @@ int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream) {
 
 long long mk_workspace_offset(mk_handle* h, const char* name, int n_pairs, int H, int W) {
   if (!h || !name) return -1;
-  const Geo g = make_geo(n_pairs, H, W);
+  const Geo g = make_geo(2 * n_pairs, n_pairs, H, W);
   uint8_t* base = reinterpret_cast<uint8_t*>(0x1000);     // fake base: only differences are used
-  Workspace w = carve(base, h->cfg, g, n_pairs);
+  Workspace w = carve(base, h->cfg, g);
   const std::unordered_map<std::string, const void*> m = {
       {"P", w.P}, {"X", w.X}, {"XN", w.XN}, {"QKV", w.QKV}, {"ATT", w.ATT}, {"H1", w.H1}, {"F", w.F}, {"T1", w.T1},
       {"S1", w.S1}, {"O1", w.O1}, {"T2", w.T2}, {"S2", w.S2}, {"O2", w.O2}, {"T3", w.T3}, {"S3", w.S3}, {"CAT", w.CAT},

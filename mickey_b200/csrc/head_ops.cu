@@ -308,6 +308,89 @@ int desc_out(const float* y, float* dsc_cm, void* dsc_x, float* nrm2, int n_img,
   return MK_OK;
 }
 
+// ------------------------------------------------------------------------------------------------------
+// Feature-bank gather (mk_forward_pairs): the per-pair operands of the matcher and the solver, taken from two banks of
+// extracted images.  Block (x, p, r): tokens [32x, 32x + 32) of pair p in role r; its image is idx_r[p] of bank r.
+//   dsc  fp32 [n, 128, N] channel-major -> dsc_x fp16 [(r*P + p)*N + tok, 384], split exactly as desc_out_kernel does
+//   kps [n,2,N], depth [n,1,N], scr [n,1,N] -> kps_out [2P,2,N], depth_out [2P,1,N], scr_out [2P,N]  (role-0 rows first)
+// The descriptor tile is transposed through shared memory: each warp reads 128-byte runs of 32 tokens of one channel and
+// writes 128-byte runs of 64 channels of one token.  An index outside [0, count) reads nothing from the bank and writes
+// zeros (bank_index_check reports it after the solve).
+// ------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+bank_gather_kernel(BankView b0, BankView b1, int P, int N, __half* __restrict__ dsc_x, float* __restrict__ kps_out,
+                   float* __restrict__ depth_out, float* __restrict__ scr_out) {
+  __shared__ float tile[128][33];
+  pdl_wait();        // launched with programmatic stream serialization: predecessors are complete past this point
+  pdl_trigger();
+  const int r = blockIdx.z, p = blockIdx.y, n0 = blockIdx.x * 32, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const BankView b = r ? b1 : b0;
+  const int img = __ldg(b.idx + p);
+  const bool ok = img >= 0 && img < b.count;
+  const long long im = ok ? img : 0, orow = (long long)r * P + p;
+  if (t < 128) {                                       // warp 0, 1: kps x, y; warp 2: depth; warp 3: scr
+    const int n = n0 + lane;
+    if (n < N) {
+      const float* src = warp < 2 ? b.kps + (im * 2 + warp) * N : (warp == 2 ? b.depth : b.scr) + im * N;
+      const float v = ok ? __ldg(src + n) : 0.f;
+      float* dst = warp < 2 ? kps_out + (orow * 2 + warp) * N : (warp == 2 ? depth_out : scr_out) + orow * N;
+      dst[n] = v;
+    }
+  }
+  const float* src = b.dsc + im * 128 * N;
+#pragma unroll
+  for (int k = 0; k < 16; ++k) {
+    const int c = warp + 8 * k, n = n0 + lane;
+    tile[c][lane] = (ok && n < N) ? __ldg(src + (long long)c * N + n) : 0.f;
+  }
+  __syncthreads();
+  for (int j = warp; j < 32 && n0 + j < N; j += 8) {
+    __half* dst = dsc_x + (orow * N + n0 + j) * 384;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int c = 64 * half + 2 * lane;
+      const float v0 = tile[c][j], v1 = tile[c + 1][j];
+      const __half h0 = __float2half_rn(v0), h1 = __float2half_rn(v1);
+      const __half2 hi = __halves2half2(h0, h1);
+      const __half2 lo = __halves2half2(__float2half_rn(v0 - __half2float(h0)), __float2half_rn(v1 - __half2float(h1)));
+      *reinterpret_cast<__half2*>(dst + c) = hi;
+      *reinterpret_cast<__half2*>(dst + 128 + c) = r ? hi : lo;      // role 0 [hi | lo | hi], role 1 [hi | hi | lo]
+      *reinterpret_cast<__half2*>(dst + 256 + c) = r ? lo : hi;
+    }
+  }
+}
+
+int bank_gather(const BankView& b0, const BankView& b1, int P, int N, void* dsc_x, float* kps_out, float* depth_out, float* scr_out,
+                cudaStream_t s) {
+  MK_CUDA_CHECK(launch_k(bank_gather_kernel, dim3(ceil_div(N, 32), P, 2), dim3(256), 0, s, b0, b1, P, N, (__half*)dsc_x, kps_out,
+                         depth_out, scr_out));
+  MK_CUDA_CHECK(cudaGetLastError());
+  return MK_OK;
+}
+
+// After the solve of mk_forward_pairs: an index outside its bank gives the batch the zero pose of the solver's status bits
+// (R = 0, t = 0, inliers = 0) and sets status bit 3.  One block; it reads only the index vectors.
+__global__ void __launch_bounds__(256)
+bank_index_check_kernel(const int* __restrict__ idx0, int n0, const int* __restrict__ idx1, int n1, int P, float* __restrict__ pose,
+                        int* __restrict__ status) {
+  pdl_wait();
+  pdl_trigger();
+  int bad = 0;
+  for (int p = threadIdx.x; p < P; p += blockDim.x) {
+    const int a = __ldg(idx0 + p), b = __ldg(idx1 + p);
+    bad |= (a < 0 || a >= n0 || b < 0 || b >= n1);
+  }
+  if (!__syncthreads_or(bad)) return;
+  for (int i = threadIdx.x; i < P * 13; i += blockDim.x) pose[i] = 0.f;
+  if (status && threadIdx.x == 0) *status |= 8;
+}
+
+int bank_index_check(const BankView& b0, const BankView& b1, int P, float* pose, int* status, cudaStream_t s) {
+  MK_CUDA_CHECK(launch_k(bank_index_check_kernel, dim3(1), dim3(256), 0, s, b0.idx, b0.count, b1.idx, b1.count, P, pose, status));
+  MK_CUDA_CHECK(cudaGetLastError());
+  return MK_OK;
+}
+
 // Fold the online-softmax partials of matcher pass 1 (EPI_LSE: float2 (max, sum) per slot, slot-major) and the dustbin
 // logit into the log2-domain log-sum-exp of every row and column of the dustbin-augmented S/T
 // (feature_matcher.py:70-77: the dustbin score is appended AFTER the division by the temperature).

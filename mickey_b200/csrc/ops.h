@@ -25,6 +25,11 @@ int kp_head_out(const float* y, const float* w_depth, const float* w_xy, const f
 int desc_out(const float* y, float* dsc_cm, void* dsc_x, float* nrm2, int n_img, int gh, int gw, int normalize, cudaStream_t s);
 int matcher_lse_reduce(const void* part_row, const void* part_col, const float* dustbin, int B, int N, int part_ld, float* lse_r,
                        float* lse_c, cudaStream_t s);
+// one bank of extracted images (kps [n,2,N], depth [n,1,N], scr [n,1,N], dsc [n,128,N]) and the image index of every pair
+struct BankView { const float *kps, *depth, *scr, *dsc; const int* idx; int count; };
+int bank_gather(const BankView& b0, const BankView& b1, int P, int N, void* dsc_x, float* kps_out, float* depth_out, float* scr_out,
+                cudaStream_t s);
+int bank_index_check(const BankView& b0, const BankView& b1, int P, float* pose, int* status, cudaStream_t s);
 
 // ransac.cu
 struct RansacParams {

@@ -223,6 +223,7 @@ class Engine:
         self._geo_state: Dict[tuple, dict] = {}
         self._graphs, self._slot = {}, {}
         self._copy_stream = None
+        self._pairs_ws = None
 
     def __del__(self):
         try:
@@ -261,6 +262,15 @@ class Engine:
 
     def prepare(self, n_pairs: int, H: int, W: int):
         """Size-dependent tables + workspace for images cropped to (H, W) (multiples of 14)."""
+        self._use_geometry(H, W)
+        if self.ws is None or self.ws_pairs < n_pairs:
+            nbytes = self.lib.mk_workspace_bytes(self.h, n_pairs, H, W)
+            self.ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            self.ws_pairs = n_pairs
+        return self.ws
+
+    def _use_geometry(self, H: int, W: int):
+        """Register the size-dependent tables of (H, W) and finalize the handle for it (kept per geometry)."""
         assert self.packed, "load_state_dict first"
         if self.geo != (H, W):
             if self.geo is not None:                       # park the outgoing geometry's workspace with its state
@@ -286,11 +296,6 @@ class Engine:
             _lib.check(self.lib.mk_finalize(self.h, H, W), "mk_finalize")
             self.geo = (H, W)
             self.ws, self.ws_pairs = gs["ws"], gs["ws_pairs"]
-        if self.ws is None or self.ws_pairs < n_pairs:
-            nbytes = self.lib.mk_workspace_bytes(self.h, n_pairs, H, W)
-            self.ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            self.ws_pairs = n_pairs
-        return self.ws
 
     @property
     def launch_count(self) -> int:
@@ -342,30 +347,91 @@ class Engine:
         return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
     # -- stages ------------------------------------------------------------------------------------------------
-    def extract(self, images: torch.Tensor):
-        """images fp32 [2B, 3, H, W] (image0 batch then image1 batch) -> kps, depth, scr, dsc.
-        H, W need not be multiples of 14: the patch gather reads only the top-left 14*(H//14) x 14*(W//14) crop
-        (reference mickey_extractor.py:46), so no cropped copy is made."""
+    @staticmethod
+    def _image_batch(images: torch.Tensor):
+        """fp32 [n, 3, H, W] or uint8 [n, H, W, 3] (RGB as decoded, SURVEY.md §8 f1) -> (contiguous images, u8, n, H, W)."""
         u8 = images.dtype == torch.uint8
-        if u8:                                           # [2B, H, W, 3] RGB as decoded (mk_extract_u8, SURVEY.md §8 f1)
+        if u8:
             assert images.dim() == 4 and images.shape[-1] == 3, "uint8 images must be [n, H, W, 3] (HWC, RGB)"
             images = images.contiguous()
             n_img, H, W, _ = images.shape
         else:
             images = images.float().contiguous()
             n_img, _, H, W = images.shape
+        return images, u8, n_img, H, W
+
+    def _outputs_of_extract(self, n_img, N):
+        dev = self.device
+        return (torch.empty(n_img, 2, N, device=dev), torch.empty(n_img, 1, N, device=dev), torch.empty(n_img, 1, N, device=dev),
+                torch.empty(n_img, self.mkcfg.desc_dim, N, device=dev))
+
+    def extract(self, images: torch.Tensor):
+        """images fp32 [2B, 3, H, W] (image0 batch then image1 batch) -> kps, depth, scr, dsc.
+        H, W need not be multiples of 14: the patch gather reads only the top-left 14*(H//14) x 14*(W//14) crop
+        (reference mickey_extractor.py:46), so no cropped copy is made."""
+        images, u8, n_img, H, W = self._image_batch(images)
         assert n_img % 2 == 0
         B, N = n_img // 2, (H // PATCH) * (W // PATCH)
         ws = self._ws_for(B, H, W)
-        dev = self.device
-        kps = torch.empty(n_img, 2, N, device=dev)
-        depth = torch.empty(n_img, 1, N, device=dev)
-        scr = torch.empty(n_img, 1, N, device=dev)
-        dsc = torch.empty(n_img, self.mkcfg.desc_dim, N, device=dev)
+        kps, depth, scr, dsc = self._outputs_of_extract(n_img, N)
         fn = self.lib.mk_extract_u8 if u8 else self.lib.mk_extract
         _lib.check(fn(self.h, _lib.ptr(images), B, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
                       _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), self._stream()), "mk_extract")
         return kps, depth, scr, dsc
+
+    # -- feature banks: extract images once, then match / solve any pairs among them ------------------------------
+    def _bank_ws(self, n_img, n_pairs, H, W):
+        """Workspace of extract_images / forward_pairs.  It is separate from forward()'s, whose buffer sets and captured
+        graphs hold that workspace's address; it grows to the largest call seen."""
+        nbytes = self.lib.mk_workspace_bytes_for(self.h, n_img, n_pairs, H, W)
+        if self._pairs_ws is None or self._pairs_ws.numel() < nbytes:
+            self._pairs_ws = None
+            self._pairs_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        return self._pairs_ws
+
+    def extract_images(self, images: torch.Tensor):
+        """Any number n >= 1 of images, fp32 [n, 3, H, W] or uint8 [n, H, W, 3] -> kps [n,2,N], depth [n,1,N], scr [n,1,N],
+        dsc [n,128,N]: per image, bit-identical to what extract() gives for that image (mk_extract_images / _u8)."""
+        images, u8, n_img, H, W = self._image_batch(images)
+        if n_img < 1:
+            raise _lib.MickeyB200Error("extract_images needs at least one image")
+        N = (H // PATCH) * (W // PATCH)
+        self._use_geometry(H, W)
+        ws = self._bank_ws(n_img, 0, H, W)
+        kps, depth, scr, dsc = self._outputs_of_extract(n_img, N)
+        fn = self.lib.mk_extract_images_u8 if u8 else self.lib.mk_extract_images
+        _lib.check(fn(self.h, _lib.ptr(images), n_img, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
+                      _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), self._stream()), "mk_extract_images")
+        return kps, depth, scr, dsc
+
+    def forward_pairs(self, bank0, idx0, bank1, idx1, K0, K1, seed: int, image_size, lean: bool = False):
+        """Match and solve the pairs (bank0[idx0[p]], bank1[idx1[p]]) in one C call (mk_forward_pairs).
+
+        bank = (kps, depth, scr, dsc) as extract_images returns it, extracted at image_size = (H, W); idx0 / idx1 int32
+        device tensors [P] that the caller has range-checked; K0 / K1 [P, 3, 3].  Returns fresh tensors: kps [2P,2,N] and
+        depth [2P,1,N] (image-0 rows first), scores / kp_scores (None when lean), final_scores, pose [P,13], best_set,
+        inlier_mask, sampled_idx, status."""
+        H, W = image_size
+        self._use_geometry(H, W)
+        P, N = idx0.numel(), bank0[0].shape[-1]
+        ws = self._bank_ws(0, P, H, W)
+        dev, c = self.device, self.mkcfg
+        out = {"kps": torch.empty(2 * P, 2, N, device=dev), "depth": torch.empty(2 * P, 1, N, device=dev),
+               "scores": None if lean else nn_empty(P, N, dev), "kp_scores": None if lean else nn_empty(P, N, dev),
+               "final_scores": nn_empty(P, N, dev), "pose": torch.empty(P, 13, device=dev),
+               "best_set": torch.empty(P, dtype=torch.int32, device=dev), "inlier_mask": torch.empty(P, c.num_sampled, device=dev),
+               "sampled_idx": torch.empty(P * c.it_matches, c.num_sampled, dtype=torch.int32, device=dev),
+               "status": torch.zeros(1, dtype=torch.int32, device=dev)}
+        K0 = K0.to(dev, torch.float32).contiguous()
+        K1 = K1.to(dev, torch.float32).contiguous()
+        seed = (int(seed) & (2 ** 64 - 1)) or 1
+        p = _lib.ptr
+        _lib.check(self.lib.mk_forward_pairs(
+            self.h, *(p(t) for t in bank0), bank0[0].shape[0], *(p(t) for t in bank1), bank1[0].shape[0], p(idx0), p(idx1),
+            p(K0), p(K1), P, C.c_ulonglong(seed), p(out["kps"]), p(out["depth"]), p(out["scores"]), p(out["kp_scores"]),
+            p(out["final_scores"]), out["final_scores"].stride(1), p(out["pose"]), p(out["best_set"]), p(out["inlier_mask"]),
+            p(out["sampled_idx"]), p(out["status"]), p(ws), ws.numel(), self._stream()), "mk_forward_pairs")
+        return out
 
     def match(self, B: int, N: int, lean: bool = False):
         """lean: only final_scores (the matrix the solver reads) is materialised; scores / kp_scores come back as None."""

@@ -12,16 +12,98 @@ forward arithmetic of its own.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+import operator
+from dataclasses import dataclass
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.nn as nn
 
+from ._lib import MickeyB200Error
 from .config import backbone_variant
 from .engine import Engine, PATCH
 from .weights import synthetic_state_dict
 
 _BUFFER_SUFFIXES = ("running_mean", "running_var", "num_batches_tracked")
+
+
+@dataclass
+class MickeyFeatures:
+    """Extractor outputs of n images (MickeyRelativePose.extract_features): a feature bank that pose_from_features pairs
+    by index.  kps [n,2,N] (pixels), depth [n,1,N], scr [n,1,N], dsc [n,128,N], fp32, in the data-dict layouts;
+    grid = (gh, gw) token grid (N = gh * gw); image_size = (H, W) of the images they were extracted from."""
+    kps: torch.Tensor
+    depth: torch.Tensor
+    scr: torch.Tensor
+    dsc: torch.Tensor
+    grid: Tuple[int, int]
+    image_size: Tuple[int, int]
+
+    def __len__(self) -> int:
+        return self.kps.shape[0]
+
+    @property
+    def device(self) -> torch.device:
+        return self.kps.device
+
+    def tensors(self):
+        return self.kps, self.depth, self.scr, self.dsc
+
+    @staticmethod
+    def cat(banks: Sequence["MickeyFeatures"]) -> "MickeyFeatures":
+        """One bank holding the images of `banks` in order (all of one geometry)."""
+        first = banks[0]
+        for b in banks[1:]:
+            if b.grid != first.grid or b.image_size != first.image_size:
+                raise MickeyB200Error(f"cannot join banks of geometry {b.image_size} and {first.image_size}")
+        if len(banks) == 1:
+            return first
+        return MickeyFeatures(*(torch.cat(ts) for ts in zip(*(b.tensors() for b in banks))), first.grid, first.image_size)
+
+
+def _host_indices(idx, name: str) -> List[int]:
+    if torch.is_tensor(idx):
+        if idx.dtype.is_floating_point or idx.dtype.is_complex or idx.dtype == torch.bool:
+            raise MickeyB200Error(f"{name} must hold integers, got {idx.dtype}")
+        return [int(v) for v in idx.detach().reshape(-1).cpu().tolist()]
+    out = []
+    for v in idx:
+        try:
+            if isinstance(v, bool):
+                raise TypeError
+            out.append(operator.index(v))
+        except TypeError:
+            raise MickeyB200Error(f"{name} must hold integers, got {v!r}") from None
+    return out
+
+
+def validate_pairs(feats0: MickeyFeatures, idx0, feats1: MickeyFeatures, idx1) -> Tuple[List[int], List[int]]:
+    """Host-side checks of a pose_from_features request, before anything is launched: integer indices inside their
+    banks, as many idx0 as idx1 (at least one pair), both banks of one geometry (the solver needs N x N square) and on
+    one device.  Returns the indices as host lists."""
+    i0, i1 = _host_indices(idx0, "idx0"), _host_indices(idx1, "idx1")
+    if len(i0) != len(i1):
+        raise MickeyB200Error(f"idx0 has {len(i0)} entries and idx1 {len(i1)}: one index of each bank per pair")
+    if not i0:
+        raise MickeyB200Error("pose_from_features needs at least one pair")
+    for name, idx, bank in (("idx0", i0, feats0), ("idx1", i1, feats1)):
+        bad = [v for v in idx if not 0 <= v < len(bank)]
+        if bad:
+            raise MickeyB200Error(f"{name} {bad[:4]} outside its bank of {len(bank)} images")
+    if feats0.grid != feats1.grid:
+        raise MickeyB200Error(f"banks of token grids {feats0.grid} and {feats1.grid}: both must come from one geometry")
+    for b in (feats0, feats1):
+        if tuple(b.grid) != (b.image_size[0] // PATCH, b.image_size[1] // PATCH):
+            raise MickeyB200Error(f"bank grid {b.grid} is not the token grid of its image size {b.image_size}")
+        N = b.grid[0] * b.grid[1]
+        if tuple(b.kps.shape[1:]) != (2, N) or tuple(b.dsc.shape[2:]) != (N,) or b.depth.shape[-1] != N or b.scr.shape[-1] != N:
+            raise MickeyB200Error(f"bank tensors {tuple(b.kps.shape)} / {tuple(b.dsc.shape)} do not match its grid {b.grid}")
+        if any(t.shape[0] != len(b) for t in b.tensors()):
+            raise MickeyB200Error("bank tensors hold different image counts")
+    devs = {t.device for b in (feats0, feats1) for t in b.tensors()}
+    if len(devs) != 1:
+        raise MickeyB200Error(f"bank tensors on several devices: {sorted(map(str, devs))}")
+    return i0, i1
 
 
 def synthetic_backbone_allowed() -> bool:
@@ -254,7 +336,7 @@ class MickeyRelativePose(nn.Module):
         w = data["final_scores"][bidx, i0, i1]
         rows = torch.cat([data["kps0"][bidx, :, i0], data["kps1"][bidx, :, i1], w[..., None],
                           data["depth_kp0"][bidx, :, i0], data["depth_kp1"][bidx, :, i1]], dim=-1)
-        if int(st["status"].item()) & 7:
+        if int(st["status"].item()) & 15:                # any zero-pose status bit (bit 3: forward_pairs index out of range)
             return [torch.zeros([0, 5])] * B
         out = []
         for b in range(B):
@@ -320,6 +402,60 @@ class MickeyRelativePose(nn.Module):
         data["t"] = t
         data["inliers"] = inliers
         return R, t
+
+    # -- feature banks: extract each image once, pose for any (i, j) among them --------------------------------------
+    @torch.no_grad()
+    def extract_features(self, images: torch.Tensor) -> MickeyFeatures:
+        """Features of n images, float [n, 3, H, W] in [0, 1] or uint8 [n, H, W, 3] RGB, in one extraction call.  Each
+        image's features are bit-identical to what forward() computes for it, whatever role it plays there."""
+        eng = self._engine()
+        if images.dtype != torch.uint8:
+            images = images.float()
+        kps, depth, scr, dsc = eng.extract_images(images.to(eng.device))
+        H, W = eng.geo
+        return MickeyFeatures(kps, depth, scr, dsc, (H // PATCH, W // PATCH), (H, W))
+
+    @torch.no_grad()
+    def pose_from_features(self, feats0: MickeyFeatures, idx0, feats1: MickeyFeatures, idx1, K_color0, K_color1,
+                           return_inliers: bool = False) -> dict:
+        """Relative pose of the P pairs (feats0[idx0[p]], feats1[idx1[p]]) from features extract_features computed.
+
+        idx0 / idx1: host lists or tensors of P image indices (validated on the host: MickeyB200Error before anything is
+        launched).  K_color0 / K_color1: [P, 3, 3] intrinsics of each pair.  Returns the data dict forward() fills for
+        those pairs (kps0/1, depth_kp0/1, scr0/1, dsc0/1, depth0/1_map, kps0/1_shape, down_factor, scores, kp_scores
+        (absent under lean_outputs), final_scores, R, t, inliers, and inliers_list with return_inliers).  One seed is
+        drawn from the torch RNG as in forward(), so under the same seed the poses equal forward() on the explicit pairs."""
+        i0, i1 = validate_pairs(feats0, idx0, feats1, idx1)
+        P = len(i0)
+        K0, K1 = torch.as_tensor(K_color0), torch.as_tensor(K_color1)
+        if tuple(K0.shape) != (P, 3, 3) or tuple(K1.shape) != (P, 3, 3):
+            raise MickeyB200Error(f"K_color0 {tuple(K0.shape)} / K_color1 {tuple(K1.shape)} must be [{P}, 3, 3]")
+        eng = self._engine()
+        if feats0.device != eng.device:
+            raise MickeyB200Error(f"features on {feats0.device}, model on {eng.device}")
+        seed = int(torch.randint(1, 2 ** 62, (1,)).item())
+        dev = eng.device
+        t0 = torch.tensor(i0, dtype=torch.int32).to(dev, non_blocking=True)
+        t1 = torch.tensor(i1, dtype=torch.int32).to(dev, non_blocking=True)
+        bank0 = tuple(t.float().contiguous() for t in feats0.tensors())
+        bank1 = tuple(t.float().contiguous() for t in feats1.tensors())
+        st = eng.forward_pairs(bank0, t0, bank1, t1, K0.float(), K1.float(), seed, feats0.image_size,
+                               lean=bool(getattr(self, "lean_outputs", False)))
+        gh, gw = feats0.grid
+        kps, depth = st["kps"], st["depth"]
+        data = {"kps0_shape": [gh, gw], "kps1_shape": [gh, gw], "down_factor": self.compute_matches.down_factor,
+                "depth0_map": depth[:P].reshape(P, 1, gh, gw), "depth1_map": depth[P:].reshape(P, 1, gh, gw),
+                "kps0": kps[:P], "kps1": kps[P:], "depth_kp0": depth[:P], "depth_kp1": depth[P:],
+                "scr0": bank0[2].index_select(0, t0.long()), "scr1": bank1[2].index_select(0, t1.long()),
+                "dsc0": bank0[3].index_select(0, t0.long()), "dsc1": bank1[3].index_select(0, t1.long())}
+        if st["scores"] is not None:
+            data["scores"], data["kp_scores"] = st["scores"], st["kp_scores"]
+        data["final_scores"] = st["final_scores"]
+        pose = st["pose"]
+        data["R"], data["t"], data["inliers"] = pose[:, :9].reshape(P, 3, 3), pose[:, 9:12].reshape(P, 1, 3), pose[:, 12:13]
+        if return_inliers:
+            data["inliers_list"] = self._inlier_list(data, st, P, gh * gw)
+        return data
 
 
 def build_model(cfg, checkpoint=""):

@@ -11,6 +11,11 @@ converts the gathered poses to submission records on its GPU (mk_pose_to_submiss
 `submission.zip` with the reference's `pose_<scene>.txt` line format, and grades the poses against the tree's ground
 truth with the reference's pose-error definitions (lib/utils/metrics.py:12-53).  With random-init weights the poses
 are noise — the run proves the plumbing and gives pairs/s end to end from JPEG files.
+
+Every val/test pair of a scene has the same image0, the scene's reference image.  `--share-reference` reads and extracts
+each reference once (ReferenceBank), extracts only the query images of a step and poses the batch from the two feature
+banks (model.pose_from_features).  The loader then leaves image0 out of its items.  Both paths draw one seed per batch,
+so under the same `--seed` they write the same submission.
 """
 import argparse
 import json
@@ -29,7 +34,7 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "compat")] if __import__("importlib").u
 from mickey_b200 import dist as mkdist                                  # noqa: E402
 from mickey_b200 import submission as mksub                             # noqa: E402
 from mickey_b200.config import mickey_cfg                               # noqa: E402
-from mickey_b200.model import build_model                               # noqa: E402
+from mickey_b200.model import MickeyFeatures, build_model               # noqa: E402
 from mickey_b200.weights import synthetic_checkpoint                    # noqa: E402
 
 
@@ -38,6 +43,30 @@ def pose_errors(R, t, T_gt):
     Rgt, tgt = T_gt[:, :3, :3], T_gt[:, :3, 3]
     cos = np.clip((np.einsum("bij,bij->b", R, Rgt) - 1) / 2, -1, 1)      # trace(R^T Rgt)
     return np.rad2deg(np.arccos(cos)), np.linalg.norm(t - tgt, axis=-1)
+
+
+class ReferenceBank:
+    """Features of the reference images the current batch uses.  A reference is read (`load(scene_root, name)`) and
+    extracted (`extract(image) -> features`) when its first pair arrives, and dropped when a batch no longer uses it: the
+    loader walks each rank's pairs scene by scene, so a scene's reference is extracted once per rank."""
+
+    def __init__(self, load, extract):
+        self.load, self.extract = load, extract
+        self.cache = {}
+        self.extracted = 0
+
+    def lookup(self, keys):
+        """keys: (scene_root, image0 name) of every pair of the batch -> (features of each distinct reference in order of
+        first use, index of every pair's reference in that list)."""
+        order = list(dict.fromkeys(keys))
+        for k in order:
+            if k not in self.cache:
+                self.cache[k] = self.extract(self.load(*k))
+                self.extracted += 1
+        for k in [k for k in self.cache if k not in order]:
+            del self.cache[k]
+        pos = {k: i for i, k in enumerate(order)}
+        return [self.cache[k] for k in order], [pos[k] for k in keys]
 
 
 def main():
@@ -50,6 +79,10 @@ def main():
     ap.add_argument("--batch_size", type=int, default=0, help="default: the reference's 12 (val) / 8 (test)")
     ap.add_argument("--workers", type=int, default=4)
     ap.add_argument("--uint8", action="store_true", help="uint8 HWC batches + fused ingest kernel (a quarter of the H2D bytes)")
+    ap.add_argument("--share-reference", action="store_true",
+                    help="extract each scene's reference image once and pose every pair from feature banks")
+    ap.add_argument("--seed", type=int, default=None,
+                    help="seed the torch RNG that the solver's per-batch seeds come from (a reproducible submission)")
     ap.add_argument("--output_root", "-o", type=Path, default=Path("results/"))
     args = ap.parse_args()
 
@@ -76,7 +109,8 @@ def main():
     cfg.TRAINING.NUM_WORKERS = args.workers
     BS = cfg.TRAINING.BATCH_SIZE
 
-    dm = DataModule(cfg, drop_last_val=False, uint8_images=args.uint8, pin_memory=True)
+    share = args.share_reference
+    dm = DataModule(cfg, drop_last_val=False, uint8_images=args.uint8, pin_memory=True, skip_image0=share)
     loader = dm.val_dataloader() if args.split == "val" else dm.test_dataloader()
     n_pairs = len(loader.dataset)
     n_steps, step_rows = mkdist.step_plan(n_pairs, world, BS)
@@ -94,6 +128,17 @@ def main():
 
     gathered = [[] for _ in range(world)]                       # rank 0: records per source rank, in step order
     h2d = 0
+    refs = None
+    if share:
+        scene_of = {str(sc.scene_root): sc for sc in loader.dataset.datasets}
+
+        def extract_reference(image):
+            nonlocal h2d
+            h2d += image.numel() * image.element_size()
+            return model.extract_features(image[None].to(dev))
+        refs = ReferenceBank(lambda root, name: scene_of[root].image(name), extract_reference)
+    if args.seed is not None:
+        torch.manual_seed(args.seed)
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     it = iter(loader)
@@ -102,11 +147,18 @@ def main():
         mine = torch.zeros(BS, 13, device=dev)
         if rows[rank] > 0:
             data = next(it)
-            for k in ("image0", "image1", "K_color0", "K_color1"):
+            for k in ("image1", "K_color0", "K_color1") if share else ("image0", "image1", "K_color0", "K_color1"):
                 data[k] = data[k].to(dev, non_blocking=True)
                 h2d += data[k].numel() * data[k].element_size()
             with torch.no_grad():
-                R, t = model(data)
+                if share:
+                    banks, idx0 = refs.lookup(list(zip(data["scene_root"], data["pair_names"][0])))
+                    queries = model.extract_features(data["image1"])
+                    data = model.pose_from_features(MickeyFeatures.cat(banks), idx0, queries, range(len(queries)),
+                                                    data["K_color0"], data["K_color1"])
+                    R, t = data["R"], data["t"]
+                else:
+                    R, t = model(data)
             mine[:rows[rank]] = mksub.pack_poses(R, t, data["inliers"])
         allp = mkdist.gather_poses(mine)                        # the ONE collective of the step ([world*BS, 13])
         if rank == 0:
@@ -127,8 +179,10 @@ def main():
         args.output_root.mkdir(parents=True, exist_ok=True)
         mksub.save_submission(results, args.output_root / "submission.zip")
         summary = {"pairs": n_pairs, "gpus": world, "batch_size": BS, "steps": n_steps, "wall_s": wall, "pairs_per_s": n_pairs / wall,
-                   "uint8_ingest": bool(args.uint8), "h2d_bytes_rank0": h2d, "valid_poses": int(recs[:, 8].sum()),
+                   "uint8_ingest": bool(args.uint8), "share_reference": share, "h2d_bytes_rank0": h2d, "valid_poses": int(recs[:, 8].sum()),
                    "scenes": len(results), "zip": str(args.output_root / "submission.zip")}
+        if share:
+            summary["references_extracted_rank0"] = refs.extracted
         if args.split == "val":
             from transforms3d.quaternions import quat2mat
             ok = recs[:, 8] > 0
