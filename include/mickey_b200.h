@@ -160,6 +160,19 @@ int mk_forward_pairs(mk_handle* h, const float* kps0_dev, const float* depth0_de
  * (np.isnan(R).any() or np.isnan(t).any() or np.isinf(t).any(), submission.py:51-52).  One D2H copy per batch. */
 int mk_pose_to_submission(const float* pose_dev, int n_pairs, double* out_dev, void* stream);
 
+/* ---- correspondences: replaces featureMatcher.get_matches_list (lib/models/MicKey/modules/utils/feature_matcher.py:19-46),
+ * batched.  scores_dev fp32 [B, N, N] with row pitch nn_pitch floats (N or 0 = contiguous; pairs N * nn_pitch floats
+ * apart), e.g. the final_scores of mk_forward.  As in the reference the last row and column are dropped: (i, j), i, j < N-1,
+ * is a match when j is the first argmax of row i, i the first argmax of column j (a NaN counts as maximal) and
+ * exp(scores[i][j]) > min_conf (exp in double, rounded to fp32).  Per pair b, sorted by score descending and equal scores
+ * by ascending i (the reference's sort leaves their order open):
+ * matches_dev int32 [B, N-1, 2] = (i, j), match_scores_dev fp32 [B, N-1], count_dev int32 [B]; entries from count[b] on
+ * are (-1, -1) / 0.  2 <= N <= 4097, finite min_conf.  ws_dev: mk_mutual_matches_ws_bytes(B, N) bytes, 8-byte aligned.
+ * Bad arguments return MK_ERR_INVALID (message via mk_last_error) and launch nothing.  Deterministic (no atomics). */
+int mk_mutual_matches(const float* scores_dev, long long nn_pitch, int B, int N, float min_conf, int* matches_dev,
+                      float* match_scores_dev, int* count_dev, void* ws_dev, long long ws_bytes, void* stream);
+long long mk_mutual_matches_ws_bytes(int B, int N);
+
 /* (Re)seed the solver's device-side generator on `stream` (used in front of a CUDA-graph replay of mk_forward
  * captured with seed = 0). */
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream);

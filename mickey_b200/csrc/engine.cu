@@ -624,6 +624,12 @@ int mk_pose_to_submission(const float* pose, int n_pairs, double* out, void* str
   return pose_to_submission(pose, n_pairs, out, (cudaStream_t)stream);
 }
 
+long long mk_mutual_matches_ws_bytes(int B, int N) { return mutual_matches_ws_bytes(B, N); }
+int mk_mutual_matches(const float* scores, long long nn_pitch, int B, int N, float min_conf, int* matches, float* match_scores,
+                      int* count, void* ws, long long ws_bytes, void* stream) {
+  return mutual_matches(scores, nn_pitch, B, N, min_conf, matches, match_scores, count, ws, ws_bytes, (cudaStream_t)stream);
+}
+
 long long mk_launch_count(mk_handle* h) { return h ? h->launches : -1; }
 
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream) {

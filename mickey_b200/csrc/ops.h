@@ -31,6 +31,11 @@ int bank_gather(const BankView& b0, const BankView& b1, int P, int N, void* dsc_
                 cudaStream_t s);
 int bank_index_check(const BankView& b0, const BankView& b1, int P, float* pose, int* status, cudaStream_t s);
 
+// matches.cu: featureMatcher.get_matches_list, batched (include/mickey_b200.h mk_mutual_matches)
+long long mutual_matches_ws_bytes(int B, int N);
+int mutual_matches(const float* scores, long long pitch, int B, int N, float min_conf, int* matches, float* match_scores,
+                   int* count, void* ws, long long ws_bytes, cudaStream_t s);
+
 // ransac.cu
 struct RansacParams {
   int it_matches, it_ransac, n_sample, n_corr, n_refine;

@@ -22,6 +22,7 @@ import torch.nn as nn
 from ._lib import MickeyB200Error
 from .config import backbone_variant
 from .engine import Engine, PATCH
+from .matches import mutual_matches
 from .weights import synthetic_state_dict
 
 _BUFFER_SUFFIXES = ("running_mean", "running_var", "num_batches_tracked")
@@ -135,6 +136,21 @@ class _ParamTree(nn.Module):
         return super().eval()
 
 
+class featureMatcher(_ParamTree):
+    """Holds the matcher's parameters (matching_mat.dustbin_score) under the reference's names and offers its
+    get_matches_list (reference feature_matcher.py:19-46), CUDA-backed (mickey_b200.matches)."""
+
+    def get_matches_list(self, scores, min_conf=0.0):
+        """MicKey's correspondences of one pair: scores [1, N, N] fp32 on the GPU (e.g. data['final_scores'][b:b+1]), any
+        strides.  Returns int64 [M, 2] (i, j) on its device, sorted by scores[0, i, j] descending, equal scores by ascending
+        i.  Like the reference, the last row and column are not candidates.  B != 1 is a ValueError (the reference supports
+        batch size 1 only; MickeyRelativePose.mutual_matches takes a batch)."""
+        if torch.is_tensor(scores) and scores.dim() == 3 and scores.shape[0] != 1:
+            raise ValueError(f"get_matches_list supports batch size 1 (as the reference does), got {tuple(scores.shape)}; "
+                             "use MickeyRelativePose.mutual_matches for a batch")
+        return mutual_matches(scores, min_conf)[0][0]
+
+
 class e2eProbabilisticProcrustesSolver:
     """Test-time metric pose solver (reference probabilisticProcrustes.py:5-20, 183-348), CUDA-backed."""
 
@@ -197,7 +213,7 @@ class ComputeCorrespondences(nn.Module):
         self.dsc_dim = cfg["MICKEY"]["DSC_HEAD"]["LAST_DIM"]
         self.down_factor = cfg["MICKEY"]["DINOV2"]["DOWN_FACTOR"]
         self.extractor = _ParamTree()
-        self.matcher = _ParamTree()
+        self.matcher = featureMatcher()
 
     def forward(self, data):
         eng = self._owner._engine()
@@ -456,6 +472,14 @@ class MickeyRelativePose(nn.Module):
         if return_inliers:
             data["inliers_list"] = self._inlier_list(data, st, P, gh * gw)
         return data
+
+    @torch.no_grad()
+    def mutual_matches(self, scores, min_conf: float = 0.0):
+        """get_matches_list (reference feature_matcher.py:19-46) of every pair of scores [B, N, N] fp32 on the GPU, e.g.
+        data['final_scores'] after forward(): a list of B int64 [M_b, 2] tensors (i, j) and a list of their B fp32 [M_b]
+        scores, each sorted by score descending, equal scores by ascending i.  Two kernel launches for the whole batch and
+        one device-to-host copy of the counts."""
+        return mutual_matches(scores, min_conf)
 
 
 def build_model(cfg, checkpoint=""):
