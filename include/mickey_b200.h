@@ -113,9 +113,14 @@ int mk_match(mk_handle* h, int n_pairs, float* scores_dev, float* kp_scores_dev,
  * Optional outputs (NULL to skip): best_set_dev int32 [n_pairs] (index into the IT_MATCHES sampled sets),
  * inlier_mask_dev fp32 [n_pairs, NUM_SAMPLED] (hard inliers of the winning set at the final pose),
  * sampled_idx_out_dev int32 [n_pairs*IT_MATCHES, NUM_SAMPLED] (the cells that were drawn),
- * hyp_scores_out_dev fp32 [n_pairs, IT_MATCHES*IT_RANSAC].  status_dev int32[1]: bit0 = not enough non-zero
- * cells, bit1 = candidate overflow (selection truncated), bit2 = non-finite hypothesis; any bit gives the reference's
- * zero pose (R = 0, t = 0, inliers = 0 for the whole batch, probabilisticProcrustes.py:331-342). */
+ * hyp_scores_out_dev fp32 [n_pairs, IT_MATCHES*IT_RANSAC].  status_dev int32[1]: bit0 = torch.multinomial would
+ * raise on the outer draw (some pair's final_scores sums to zero, holds a NaN, an inf or a negative cell, or has
+ * fewer than NUM_SAMPLED cells), bit1 = a stream's candidate list was truncated or came short (probability < 1e-13),
+ * bit2 = non-finite hypothesis; any of these bits gives the reference's zero pose (R = 0, t = 0, inliers = 0 for the
+ * whole batch, probabilisticProcrustes.py:331-342).  A pair with 0 < positive cells < NUM_SAMPLED is not a failure,
+ * as in the reference: every positive cell is drawn and the lowest-index zero cells fill the set.  When such a set
+ * holds fewer than 3 positive weights, the inner draw takes the positive ones and fills the triple with the entries
+ * that follow them in the set, cyclically (ATen fills with zero-weight entries too, in an unspecified order). */
 int mk_solve_pose(mk_handle* h, const float* final_scores_dev, long long nn_pitch, const float* kps_dev, const float* depth_dev,
                   const float* K0_dev, const float* K1_dev, int n_pairs, int n_kpts, unsigned long long seed,
                   const int* outer_idx_dev, const int* inner_idx_dev, float* pose_dev, int* best_set_dev,

@@ -134,20 +134,28 @@ __device__ __forceinline__ void for_each_cell(const CellView& cv, long long chun
   }
 }
 
+// p > 0 and finite, subnormals included (an integer test: it does not depend on how the compiler treats subnormals)
+__device__ __forceinline__ bool positive_finite(float pv) { return __float_as_uint(pv) - 1u < 0x7f7fffffu; }
+
+// Besides the histogram, pass A flags the cells torch.multinomial rejects: NaN (either sign bit), +-inf and p < 0
+// (-0 is a zero).  Status bit 0 then gives the reference's zero pose (probabilisticProcrustes.py:331-342).
 template <int MODE>
 __global__ void __launch_bounds__(SAMP_THREADS)
-sampler_phist_kernel(const float* __restrict__ fs, int N, long long pitch, unsigned int* __restrict__ hist) {
+sampler_phist_kernel(const float* __restrict__ fs, int N, long long pitch, unsigned int* __restrict__ hist, int* __restrict__ status) {
   __shared__ unsigned int h[HBINS];
   for (int i = threadIdx.x; i < HBINS; i += SAMP_THREADS) h[i] = 0;
   __syncthreads();
   const int b = blockIdx.y;
   const CellView cv{fs + (long long)b * N * pitch, N, pitch};
   const long long n_chunks = cv.n_chunks(MODE);
+  bool invalid = false;
   for (long long chunk = blockIdx.x; chunk < n_chunks; chunk += gridDim.x)      // grid = whole waves of resident blocks
     for_each_cell<MODE>(cv, chunk, [&](long long, float pv) {
-      if (pv > 0.f) atomicAdd(&h[__float_as_uint(pv) >> 20], 1u);
+      const uint32_t u = __float_as_uint(pv);
+      if (positive_finite(pv)) atomicAdd(&h[u >> 20], 1u);
+      else invalid |= (u & 0x7fffffffu) != 0u;
     });
-  __syncthreads();
+  if (__syncthreads_or(invalid) && threadIdx.x == 0) atomicOr(status, 1);
   unsigned int* dst = hist + (long long)b * HBINS;
   for (int i = threadIdx.x; i < HBINS; i += SAMP_THREADS)
     if (h[i]) atomicAdd(dst + i, h[i]);
@@ -158,14 +166,14 @@ sampler_phist_kernel(const float* __restrict__ fs, int N, long long pitch, unsig
 // expected number of survivors f(tau) = sum_bins count * (1 - exp(-lower_edge / tau)) is evaluated on the grid of
 // bin edges and the largest tau with f(tau) >= n_sample + 8 sqrt(n_sample) + 16 is taken (f decreases in tau).  The
 // number of survivors of a stream is a sum of independent Bernoullis (variance <= mean), so fewer than n_sample
-// survive with probability < 1e-13; that event is reported through status bit 1 like "not enough nonzero cells".
+// survive with probability < 1e-13; pass C reports that event through status bit 1.
 // One 1024-thread block per pair runs a 33-ary search: each round, warp w evaluates f at its own grid point (64 bins
 // per lane, fixed-order shuffle reduction), so three rounds replace eleven bisection steps of block-wide reductions.
 constexpr int TAU_THREADS = 1024;
 
 __global__ void __launch_bounds__(TAU_THREADS)
-sampler_tau_kernel(const unsigned int* __restrict__ hist, int n_sample, int* __restrict__ thr, float* __restrict__ inv_tau,
-                   int* __restrict__ status) {
+sampler_tau_kernel(const unsigned int* __restrict__ hist, long long cells, int n_sample, int* __restrict__ thr,
+                   float* __restrict__ inv_tau, int* __restrict__ status) {
   pdl_wait();        // launched with programmatic stream serialization: predecessors are complete past this point
   pdl_trigger();
   __shared__ float cc[HBINS], ee[HBINS];          // counts and lower edges of the occupied bins, in bin order
@@ -173,10 +181,11 @@ sampler_tau_kernel(const unsigned int* __restrict__ hist, int n_sample, int* __r
   __shared__ float fw[32];
   const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const unsigned int* h = hist + (long long)b * HBINS;
-  // compact the occupied bins (a few hundred of the 2048): thread t owns bins 2t, 2t+1; bin 0 (p == 0) and the
-  // inf / nan bins >= 2040 never take part
+  // compact the occupied bins (a few hundred of the 2048): thread t owns bins 2t, 2t+1.  Pass A histograms positive
+  // finite p only, so bin 0 holds 0 < p < 2^-129 (its lower edge 0 adds nothing to f) and the inf / nan bins >= 2040
+  // stay empty.
   const int b0 = 2 * t, b1 = 2 * t + 1;
-  const unsigned int c0 = (b0 >= 1 && b0 < HBINS - 8) ? h[b0] : 0u, c1 = (b1 < HBINS - 8) ? h[b1] : 0u;
+  const unsigned int c0 = (b0 < HBINS - 8) ? h[b0] : 0u, c1 = (b1 < HBINS - 8) ? h[b1] : 0u;
   const int k = (c0 > 0) + (c1 > 0);
   int incl = k;
 #pragma unroll
@@ -229,9 +238,10 @@ sampler_tau_kernel(const unsigned int* __restrict__ hist, int n_sample, int* __r
     const bool all = (lo < 8);
     thr[b] = all ? 1 : lo;
     inv_tau[b] = all ? __int_as_float(0x7f800000) : 1.0f / tau;
-    // zero-probability cells may never be drawn (ATen raises in that case and the reference's try/except returns
-    // the zero pose, probabilisticProcrustes.py:331-342)
-    if (nonzero < (float)n_sample) atomicOr(status, 1);
+    // torch.multinomial without replacement raises on a row that sums to zero and when n_sample exceeds the row
+    // length; the reference's try/except then returns the zero pose (probabilisticProcrustes.py:331-342).  With
+    // 0 < positive cells < n_sample it does not raise: pass C draws every positive cell and fills with zero cells.
+    if (nonzero == 0.f || cells < (long long)n_sample) atomicOr(status, 1);
   }
 }
 
@@ -253,7 +263,7 @@ __device__ __noinline__ void collect_refine(const Philox& rng, long long e, floa
       const float u = u_from_prefix(prefix, r2.x);
       if (u <= uth) {
         const uint32_t k = race_key(pv, u);
-        if ((int)(k >> 20) >= T) {
+        if (T <= 1 || (int)(k >> 20) >= T) {               // all-candidates mode: even a key that underflows to 0
           const long long s = (long long)b * IM + stream;
           const unsigned int slot = atomicAdd(cnt + s, 1u);
           if (slot < (unsigned)cap) cand[s * cap + slot] = ((unsigned long long)k << 32) | (uint32_t)e;
@@ -276,7 +286,7 @@ sampler_collect_kernel(const float* __restrict__ fs, int N, long long pitch, int
   const float inv_tau = inv_tau_p[b];
   const CellView cv{fs + (long long)b * N * pitch, N, pitch};
   auto cell = [&](long long e, float pv) {
-    if (!(pv > 0.f)) return;
+    if (!positive_finite(pv)) return;
     // u <= (1 - exp(-y)) * (1 + 2^-10) + 2^-30 with y = p / tau: a superset of the exact condition.  For small y
     // 1 - exp(-y) <= y is used instead (1 - q would cancel catastrophically in fp32).
     const float y = pv * inv_tau;
@@ -392,9 +402,12 @@ template <int E>
 __device__ __forceinline__ void select_run(const unsigned long long* __restrict__ src, int n, int n_sample, int* __restrict__ dst,
                                            unsigned int* hist, uint32_t* sel, int* ctrl) {
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  // padding is masked out rather than told apart by value: in all-candidates mode a real candidate can be 0
+  // (cell 0 with a key that underflowed)
   unsigned long long v[E];
+  auto valid = [&](int r) { return t + SEL_THREADS * r < n; };
 #pragma unroll
-  for (int r = 0; r < E; ++r) v[r] = (t + SEL_THREADS * r < n) ? src[t + SEL_THREADS * r] : 0ull;   // 0 < every real candidate
+  for (int r = 0; r < E; ++r) v[r] = valid(r) ? src[t + SEL_THREADS * r] : 0ull;
   // ---- 1. radix select of the n_sample-th largest
   unsigned long long prefix = 0;         // bytes already fixed (value of v >> (shift + 8) of the boundary element)
   int need = n_sample;                   // how many must still come out of the elements matching the prefix
@@ -406,7 +419,7 @@ __device__ __forceinline__ void select_run(const unsigned long long* __restrict_
     __syncthreads();
 #pragma unroll
     for (int r = 0; r < E; ++r)
-      if (shift == 56 || (v[r] >> (shift + 8)) == prefix) atomicAdd(&hist[(unsigned)(v[r] >> shift) & 0xffu], 1u);
+      if (valid(r) && (shift == 56 || (v[r] >> (shift + 8)) == prefix)) atomicAdd(&hist[(unsigned)(v[r] >> shift) & 0xffu], 1u);
     __syncthreads();
     if (warp == 0) {                     // suffix counts over the 256 bins: lane owns bins [8 lane, 8 lane + 8)
       unsigned int c[8], mine = 0;
@@ -437,7 +450,7 @@ __device__ __forceinline__ void select_run(const unsigned long long* __restrict_
   __syncthreads();
 #pragma unroll
   for (int r = 0; r < E; ++r)
-    if (v[r] != 0ull && (v[r] >> shift) >= bound) { const int slot = atomicAdd(&ctrl[3], 1); if (slot < 4 * SEL_THREADS) sel[slot] = (uint32_t)v[r]; }
+    if (valid(r) && (v[r] >> shift) >= bound) { const int slot = atomicAdd(&ctrl[3], 1); if (slot < 4 * SEL_THREADS) sel[slot] = (uint32_t)v[r]; }
   __syncthreads();
   const int got = min(ctrl[3], 4 * SEL_THREADS);
   uint32_t c4[4];
@@ -450,28 +463,75 @@ __device__ __forceinline__ void select_run(const unsigned long long* __restrict_
     if (4 * t + r < n_sample) dst[4 * t + r] = (4 * t + r < got) ? (int)c4[r] : 0;
 }
 
+// Fewer candidates than n_sample (n < n_sample <= 2048).  In all-candidates mode they are every positive cell, and
+// torch.multinomial's draw is those cells plus n_sample - n zero-probability cells (keys 0 / Exp(1) = 0; which ones is
+// implementation-defined).  The rule here: the lowest cell indices that are not candidates.  The first 2048 cells
+// hold at least 2048 - n of them; with fewer than n_sample cells in the matrix (status bit 0) the rest is cell 0.
+// The draw is sorted ascending by cell index like a full one.  Out of line: inlined, this rare path took the kernel
+// from 64 to 87 registers (one 512-thread block per SM instead of two).
+__device__ __noinline__ void select_fill(const unsigned long long* __restrict__ src, int n, int n_sample, long long cells,
+                                         int* __restrict__ dst, unsigned int* taken, uint32_t* sel, int* ctrl) {
+  constexpr int SZ = 4 * SEL_THREADS;
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  for (int i = t; i < SZ / 32; i += SEL_THREADS) taken[i] = 0u;
+  __syncthreads();
+  for (int i = t; i < n; i += SEL_THREADS) {
+    const uint32_t c = (uint32_t)src[i];
+    sel[i] = c;
+    if (c < (uint32_t)SZ) atomicOr(&taken[c >> 5], 1u << (c & 31));
+  }
+  __syncthreads();
+  // thread t looks at cells 4t .. 4t+3; the free ones get consecutive ranks in cell order (block-wide exclusive scan)
+  bool fr[4];
+  int k = 0;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const uint32_t c = 4 * t + r;
+    fr[r] = (long long)c < cells && !((taken[c >> 5] >> (c & 31)) & 1u);
+    k += fr[r];
+  }
+  int incl = k;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int x = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += x; }
+  if (lane == 31) ctrl[warp] = incl;
+  __syncthreads();
+  int rank = n + incl - k;
+  for (int w = 0; w < warp; ++w) rank += ctrl[w];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+    if (fr[r]) { if (rank < n_sample) sel[rank] = 4 * t + r; ++rank; }
+  int got = n;
+  for (int w = 0; w < SEL_THREADS / 32; ++w) got += ctrl[w];
+  got = min(got, n_sample);
+  __syncthreads();
+  uint32_t c4[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) c4[r] = (4 * t + r < got) ? sel[4 * t + r] : 0xffffffffu;
+  __syncthreads();
+  sort2048_u32(c4, sel, t);
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+    if (4 * t + r < n_sample) dst[4 * t + r] = (4 * t + r < got) ? (int)c4[r] : 0;
+}
+
 template <int CAP>
 __global__ void __launch_bounds__(SEL_THREADS)
-sampler_select_kernel(const unsigned long long* __restrict__ cand, const unsigned int* __restrict__ cnt, int n_sample,
-                      int* __restrict__ idx_out, int* __restrict__ status) {
+sampler_select_kernel(const unsigned long long* __restrict__ cand, const unsigned int* __restrict__ cnt, int n_sample, int IM,
+                      const int* __restrict__ thr, long long cells, int* __restrict__ idx_out, int* __restrict__ status) {
   pdl_wait();        // launched with programmatic stream serialization: predecessors are complete past this point
   pdl_trigger();
   __shared__ unsigned int hist[256];
   __shared__ uint32_t sel[4 * SEL_THREADS];
-  __shared__ int ctrl[4];
+  __shared__ int ctrl[SEL_THREADS / 32];
   const long long s = blockIdx.x;
   const unsigned int n_raw = cnt[s];
   const int n = (int)min(n_raw, (unsigned)CAP);
-  if (threadIdx.x == 0) {
-    if (n_raw > (unsigned)CAP) atomicOr(status, 2);     // candidate buffer overflow (selection truncated)
-    if (n < n_sample) atomicOr(status, 1);
-  }
+  // bit 1: the candidate buffer overflowed (selection truncated), or a thresholded stream came short of n_sample
+  // (probability < 1e-13, see sampler_tau_kernel)
+  if (threadIdx.x == 0 && (n_raw > (unsigned)CAP || (n < n_sample && thr[s / IM] > 1))) atomicOr(status, 2);
   const unsigned long long* src = cand + s * CAP;
   int* dst = idx_out + s * n_sample;
-  if (n < n_sample) {                                   // not enough candidates: status bit 1 is set, the pose is zeroed
-    for (int i = threadIdx.x; i < n_sample; i += SEL_THREADS) dst[i] = (i < n) ? (int)(uint32_t)src[i] : 0;
-    return;
-  }
+  if (n < n_sample) { select_fill(src, n, n_sample, cells, dst, hist, sel, ctrl); return; }
   if (n <= 4 * SEL_THREADS) select_run<4>(src, n, n_sample, dst, hist, sel, ctrl);
   else if (n <= 8 * SEL_THREADS) select_run<8>(src, n, n_sample, dst, hist, sel, ctrl);
   else select_run<16>(src, n, n_sample, dst, hist, sel, ctrl);
@@ -505,18 +565,19 @@ int sample_outer(const float* final_scores, int B, int N, long long pitch, int I
                    : (pitch % 4 == 0 && pitch >= 4LL * spr && aligned && rpc >= 1) ? MODE_ROW_VEC : MODE_SCALAR;
   const long long chunks = (mode == MODE_ROW_VEC) ? (N + rpc - 1) / rpc : (cells + SAMP_ELEMS_PER_BLOCK - 1) / SAMP_ELEMS_PER_BLOCK;
   dim3 grid((unsigned)min(chunks, 65535LL * 16), B);
-  if (mode == MODE_FLAT_VEC) sampler_phist_kernel<MODE_FLAT_VEC><<<grid, SAMP_THREADS, 0, st>>>(final_scores, N, pitch, hist);
-  else if (mode == MODE_ROW_VEC) sampler_phist_kernel<MODE_ROW_VEC><<<grid, SAMP_THREADS, 0, st>>>(final_scores, N, pitch, hist);
-  else sampler_phist_kernel<MODE_SCALAR><<<grid, SAMP_THREADS, 0, st>>>(final_scores, N, pitch, hist);
+  if (mode == MODE_FLAT_VEC) sampler_phist_kernel<MODE_FLAT_VEC><<<grid, SAMP_THREADS, 0, st>>>(final_scores, N, pitch, hist, status);
+  else if (mode == MODE_ROW_VEC) sampler_phist_kernel<MODE_ROW_VEC><<<grid, SAMP_THREADS, 0, st>>>(final_scores, N, pitch, hist, status);
+  else sampler_phist_kernel<MODE_SCALAR><<<grid, SAMP_THREADS, 0, st>>>(final_scores, N, pitch, hist, status);
   MK_CUDA_CHECK(cudaGetLastError());
-  MK_CUDA_CHECK(launch_k(sampler_tau_kernel, dim3(B), dim3(TAU_THREADS), 0, st, hist, n_sample, thr, inv_tau, status));
+  MK_CUDA_CHECK(launch_k(sampler_tau_kernel, dim3(B), dim3(TAU_THREADS), 0, st, hist, cells, n_sample, thr, inv_tau, status));
   MK_CUDA_CHECK(cudaGetLastError());
   if (mode == MODE_FLAT_VEC) MK_CUDA_CHECK(launch_k(sampler_collect_kernel<MODE_FLAT_VEC>, grid, dim3(SAMP_THREADS), 0, st, final_scores, N, pitch, IM, seed, thr, inv_tau, cand, cnt, CAND_CAP));
   else if (mode == MODE_ROW_VEC) MK_CUDA_CHECK(launch_k(sampler_collect_kernel<MODE_ROW_VEC>, grid, dim3(SAMP_THREADS), 0, st, final_scores, N, pitch, IM, seed, thr, inv_tau, cand, cnt, CAND_CAP));
   else MK_CUDA_CHECK(launch_k(sampler_collect_kernel<MODE_SCALAR>, grid, dim3(SAMP_THREADS), 0, st, final_scores, N, pitch, IM, seed, thr, inv_tau, cand, cnt, CAND_CAP));
   MK_CUDA_CHECK(cudaGetLastError());
   if (n_sample > 4 * SEL_THREADS) { set_last_error("NUM_SAMPLED_MATCHES %d too large", n_sample); return MK_ERR_UNSUPPORTED; }
-  MK_CUDA_CHECK(launch_k(sampler_select_kernel<CAND_CAP>, dim3((unsigned)streams), dim3(SEL_THREADS), 0, st, cand, cnt, n_sample, idx_out, status));
+  MK_CUDA_CHECK(launch_k(sampler_select_kernel<CAND_CAP>, dim3((unsigned)streams), dim3(SEL_THREADS), 0, st, cand, cnt, n_sample, IM,
+                         (const int*)thr, cells, idx_out, status));
   MK_CUDA_CHECK(cudaGetLastError());
   return MK_OK;
 }
