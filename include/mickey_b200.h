@@ -178,6 +178,44 @@ int mk_mutual_matches(const float* scores_dev, long long nn_pitch, int B, int N,
                       float* match_scores_dev, int* count_dev, void* ws_dev, long long ws_bytes, void* stream);
 long long mk_mutual_matches_ws_bytes(int B, int N);
 
+/* ---- training loss: replaces the non-differentiated part of MetricPoseLoss.RANSAC_vectorized
+ * (lib/models/MicKey/modules/loss/loss_class.py:79-329); mickey_b200/loss.py adds the differentiable tail in autograd.
+ * No handle: the calls only need the caller's tensors and a workspace.
+ *
+ * mk_loss_search: the outer draw, the inner draws and the refinement search.
+ * final_scores_dev fp32 [B, N, N] with row pitch nn_pitch floats (N or 0 = contiguous); kps0/kps1 [B,2,N] px coords,
+ * depth0/depth1 [B,1,N], K0/K1 fp32 [B,3,3] (K_color0/1).  it_matches / it_ransac / n_sample / n_corr / n_ref / th_ref are
+ * GENERATE_HYPOTHESES.IT_MATCHES / IT_RANSAC, SAMPLER.NUM_SAMPLES_MATCHES (S), NUM_CORR_3d3d (C), NUM_REF_STEPS and
+ * INLIER_REF_TH; S a multiple of 256 up to 2048, 1 <= C <= 16.
+ * outer_idx_dev int32 [B*IM, S] / inner_idx_dev int32 [B*IM*IR, C] (positions 0..S-1 in the set): when non-NULL they replace
+ * the two random draws (:138, :159); they must hold valid indices.  seed: the draws' counter-based generator.
+ * Out: sampled_idx_out_dev int32 [B*IM, S] (the drawn cells; the injected ones when given), inner_idx_out_dev int32
+ * [B*IM*IR, C] (in draw order), inliers_out_dev uint32 [B*IM*IR, S/32]: inliers_final of every hypothesis (:168-191), bit
+ * (i & 31) of word i / 32 for set position i.  status_dev int32[1]: bit0 = the outer torch.multinomial would raise (as
+ * mk_solve_pose), bit1 = a candidate list was truncated (probability < 1e-13), MK_LOSS_STATUS_PRECHECK = the batch holds a
+ * NaN, an inf or a negative cell (:126-131; the search is skipped, inliers 0, inner -1), MK_LOSS_STATUS_INNER = a set's
+ * scores sum to zero, so the inner torch.multinomial would raise.  Any of these bits gives the reference's zero result
+ * (num_valid_h = 0).  A set with fewer than C positive scores is not a failure, as in torch: the positive entries are drawn
+ * first and the entries that follow the last pick, cyclically, fill the rest.  Workspace: mk_loss_search_ws_bytes(B, IM).
+ *
+ * mk_loss_gradient: probs_grad_dev fp32 [B, N, N] contiguous = mask_b (sum_i [cell in S_i] loss_i - count baseline_b) / IM
+ * (:251-261, :299-316) from sampled_idx_dev int32 [B*IM, S] (any order), loss_value_dev fp32 [B*IM], baseline_dev fp32 [B]
+ * and mask_topk_dev fp32 [B].  Summed in iteration order without atomics (deterministic); cells never drawn are 0.
+ * Workspace: mk_loss_gradient_ws_bytes(B, IM, S).
+ * Both calls reject bad arguments with MK_ERR_INVALID (message via mk_last_error) before launching anything. */
+#define MK_LOSS_STATUS_PRECHECK 16
+#define MK_LOSS_STATUS_INNER 32
+int mk_loss_search(const float* final_scores_dev, long long nn_pitch, const float* kps0_dev, const float* depth0_dev,
+                   const float* kps1_dev, const float* depth1_dev, const float* K0_dev, const float* K1_dev, int B, int N,
+                   int it_matches, int it_ransac, int n_sample, int n_corr, int n_ref, float th_ref, unsigned long long seed,
+                   const int* outer_idx_dev, const int* inner_idx_dev, int* sampled_idx_out_dev, int* inner_idx_out_dev,
+                   unsigned int* inliers_out_dev, int* status_dev, void* ws_dev, long long ws_bytes, void* stream);
+long long mk_loss_search_ws_bytes(int B, int it_matches);
+int mk_loss_gradient(const int* sampled_idx_dev, const float* loss_value_dev, const float* baseline_dev, const float* mask_topk_dev,
+                     int B, int N, int it_matches, int n_sample, float* probs_grad_dev, void* ws_dev, long long ws_bytes,
+                     void* stream);
+long long mk_loss_gradient_ws_bytes(int B, int it_matches, int n_sample);
+
 /* (Re)seed the solver's device-side generator on `stream` (used in front of a CUDA-graph replay of mk_forward
  * captured with seed = 0). */
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream);

@@ -97,6 +97,14 @@ EXPORTS = {
     "mk_mutual_matches": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
     "mk_mutual_matches_ws_bytes": (C.c_longlong, [C.c_int, C.c_int]),
+    "mk_loss_search": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                 C.c_ulonglong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_loss_search_ws_bytes": (C.c_longlong, [C.c_int, C.c_int]),
+    "mk_loss_gradient": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                   C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_loss_gradient_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int]),
     "mk_pose_to_submission": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "mk_launch_count": (C.c_longlong, [C.c_void_p]),
     "mk_set_seed": (C.c_int, [C.c_void_p, C.c_ulonglong, C.c_void_p]),

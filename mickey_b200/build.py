@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_C")
 LIB = os.path.join(OUT_DIR, "libmickey_b200.so")
-SOURCES = ["gemm.cu", "vit_ops.cu", "attention_tc.cu", "head_ops.cu", "ransac.cu", "io_ops.cu", "matches.cu", "engine.cu"]
+SOURCES = ["gemm.cu", "vit_ops.cu", "attention_tc.cu", "head_ops.cu", "ransac.cu", "io_ops.cu", "matches.cu", "loss.cu", "engine.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

@@ -630,6 +630,23 @@ int mk_mutual_matches(const float* scores, long long nn_pitch, int B, int N, flo
   return mutual_matches(scores, nn_pitch, B, N, min_conf, matches, match_scores, count, ws, ws_bytes, (cudaStream_t)stream);
 }
 
+long long mk_loss_search_ws_bytes(int B, int IM) { return (B > 0 && IM > 0) ? loss_search_ws_bytes(B, IM) : 0; }
+int mk_loss_search(const float* final_scores, long long nn_pitch, const float* kps0, const float* depth0, const float* kps1,
+                   const float* depth1, const float* K0, const float* K1, int B, int N, int it_matches, int it_ransac,
+                   int n_sample, int n_corr, int n_ref, float th_ref, unsigned long long seed, const int* outer_idx,
+                   const int* inner_idx, int* sampled_idx_out, int* inner_idx_out, unsigned int* inliers_out, int* status,
+                   void* ws, long long ws_bytes, void* stream) {
+  return loss_search(final_scores, nn_pitch, kps0, depth0, kps1, depth1, K0, K1, B, N, it_matches, it_ransac, n_sample, n_corr,
+                     n_ref, th_ref, seed, outer_idx, inner_idx, sampled_idx_out, inner_idx_out, inliers_out, status, ws, ws_bytes,
+                     (cudaStream_t)stream);
+}
+long long mk_loss_gradient_ws_bytes(int B, int it_matches, int n_sample) { return loss_gradient_ws_bytes(B, it_matches, n_sample); }
+int mk_loss_gradient(const int* sampled_idx, const float* loss_value, const float* baseline, const float* mask_topk, int B, int N,
+                     int it_matches, int n_sample, float* probs_grad, void* ws, long long ws_bytes, void* stream) {
+  return loss_gradient(sampled_idx, loss_value, baseline, mask_topk, B, N, it_matches, n_sample, probs_grad, ws, ws_bytes,
+                       (cudaStream_t)stream);
+}
+
 long long mk_launch_count(mk_handle* h) { return h ? h->launches : -1; }
 
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream) {

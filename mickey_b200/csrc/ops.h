@@ -47,11 +47,22 @@ int seed_advance(unsigned long long* s, cudaStream_t st);
 size_t sampler_workspace_bytes(int B, int IM);
 // final_scores: [B][N][N] with row pitch `pitch` floats (N = contiguous)
 int sample_outer(const float* final_scores, int B, int N, long long pitch, int IM, int n_sample, const unsigned long long* seed,
-                 void* ws, int* idx_out, int* status, cudaStream_t st);
+                 void* ws, int* idx_out, int* status, cudaStream_t st, int invalid_bits = 1);
 int ransac_solve(const float* final_scores, long long pitch, const float* kps0, const float* d0, const float* kps1, const float* d1,
                  const float* K0, const float* K1, int B, int N, const RansacParams& rp, const int* outer_idx,
                  const int* inner_idx, float* hyp_scores, float* hyp_Rt, int* counters, float* pose,
                  int* best_set, float* inl_mask, int* best_hyp, cudaStream_t st);
 constexpr int SOLVER_COUNTER_BASE = 4;      // counters: [0] status bits, [1] pairs finished, [4 + b] blocks of pair b finished
+
+// loss.cu: MetricPoseLoss's draws, refinement search and REINFORCE gradient (include/mickey_b200.h mk_loss_search)
+constexpr int LOSS_MAX_C = 16, LOSS_MAX_S = 2048;
+long long loss_search_ws_bytes(int B, int IM);
+int loss_search(const float* fs, long long pitch, const float* kps0, const float* d0, const float* kps1, const float* d1,
+                const float* K0, const float* K1, int B, int N, int IM, int IR, int S, int C, int n_ref, float th_ref,
+                unsigned long long seed, const int* outer_idx, const int* inner_idx, int* sampled_out, int* inner_out,
+                uint32_t* inl_out, int* status, void* ws, long long ws_bytes, cudaStream_t st);
+long long loss_gradient_ws_bytes(int B, int IM, int S);
+int loss_gradient(const int* sampled, const float* loss_value, const float* baseline, const float* mask, int B, int N, int IM,
+                  int S, float* grad, void* ws, long long ws_bytes, cudaStream_t st);
 
 }  // namespace mk
