@@ -17,8 +17,8 @@ from mickey_b200.config import mickey_cfg
 from mickey_b200.model import MickeyRelativePose
 from mickey_b200.weights import synthetic_state_dict
 from oracle import mickey_oracle as mo
-from tests import draws
-from tests.common import rotation_angle_deg, synthetic_pair
+from tests import draws, stages
+from tests.common import synthetic_pair
 from tests.gpu_util import stream
 
 pytestmark = pytest.mark.gpu
@@ -26,7 +26,7 @@ DEV = "cuda"
 H, W = 720, 540
 N_S = 2048
 GEOS = {"C3": ("vitb", 32, 16, 64), "C2": ("vits", 1, 8, 64), "L": ("vitl", 1, 20, 100)}
-SEED = 0x5EED5EED12345677
+SEED = stages.SEED
 
 
 def _model(variant, im, ir, seed=3):
@@ -36,24 +36,16 @@ def _model(variant, im, ir, seed=3):
     return cfg, model.cuda().eval()
 
 
-class Prod:
+class Prod(stages.Solved):
     """compute_matches at 720x540, then the solver with its own draws."""
 
     def __init__(self, name):
         variant, B, im, ir = GEOS[name]
-        self.name, self.B, self.im, self.ir = name, B, im, ir
-        self.cfg, self.model = _model(variant, im, ir)
-        self.data = {k: v.to(DEV) for k, v in synthetic_pair(B, H, W, seed=17).items()}
+        cfg, model = _model(variant, im, ir)
+        data = {k: v.to(DEV) for k, v in synthetic_pair(B, H, W, seed=17).items()}
         with torch.no_grad():
-            self.model.compute_matches(self.data)
-            self.data["final_scores"] = self.data.pop("_final_scores_fused")        # as forward() does
-            self.R, self.t, self.inl = self.model.e2e_Procrustes.estimate_pose_vectorized(self.data, seed=SEED)
-        torch.cuda.synchronize()
-        self.res = self.data["_solver"]
-        eng = self.model._engine()
-        self.hyp_Rt = eng.ws_view("hyp_Rt", torch.float32, (B * im * ir, 12)).clone()
-        self.fs = self.data["final_scores"]
-        self.N = self.fs.shape[-1]
+            model.compute_matches(data)
+        super().__init__(name, cfg, model, data, B, im, ir)
 
 
 @pytest.fixture(scope="module", params=list(GEOS))
@@ -64,88 +56,14 @@ def prod(request):
     torch.cuda.empty_cache()
 
 
-def _band_all(fs_b, got, b, IM, seed, label):
-    """Band-check IM streams of pair b; returns (max n_diff, max n_band)."""
-    p = fs_b.reshape(-1).double()
-    worst_diff = worst_band = 0
-    for s, key in draws.outer_keys(p, seed, b, range(IM)):
-        r = draws.band_check(got[s], key, N_S)
-        assert r["ok"], (label, b, s, r)
-        worst_diff, worst_band = max(worst_diff, r["n_diff"]), max(worst_band, r["n_band"])
-    return worst_diff, worst_band
-
-
 def test_production_outer_draw_is_the_race(prod):
     if prod.name == "C3":
         assert prod.fs.stride(1) == 1952                    # the matcher's padded pitch: ROW_VEC loads
-    assert int(prod.res["status"].item()) == 0
-    got = prod.res["sampled_idx"].long().reshape(prod.B, prod.im, N_S)
-    diff = band = 0
-    for b in range(prod.B):
-        d, n = _band_all(prod.fs[b].contiguous(), got[b], b, prod.im, SEED, prod.name)
-        diff, band = max(diff, d), max(band, n)
-    print(f"\n[{prod.name}] {prod.B * prod.im} streams: max cells differing from fp64 {diff}, max cells in band {band}")
-
-
-def _hyp_reference(prod, inner):
-    """fp64 oracle with the kernel's outer draw and the given inner draw injected (on the GPU)."""
-    d = prod.data
-    trace = {}
-    Ro, to, _ = mo.solve_pose(prod.fs.double(), d["kps0"].double(), d["depth_kp0"].double(), d["kps1"].double(),
-                              d["depth_kp1"].double(), d["K_color0"].double(), d["K_color1"].double(), prod.cfg,
-                              outer_idx=prod.res["sampled_idx"].long(), inner_idx=inner, trace=trace)
-    return Ro, to, trace
+    stages.outer_draws_are_the_race(prod)
 
 
 def test_production_inner_draws_are_restated(prod):
-    B, im, ir = prod.B, prod.im, prod.ir
-    outer = prod.res["sampled_idx"].long()                              # [B*im, n_s]
-    b_of = torch.arange(B, device=DEV).repeat_interleave(im)
-    s_in = torch.arange(im, device=DEV).repeat(B)
-    w = prod.fs.reshape(B, -1)[b_of[:, None], outer]
-    idx, amb = draws.inner_draw(draws.inner_cdf(w.float()), SEED, b_of, s_in, ir)
-    inner = idx.reshape(-1, 3)
-    Ro, to, tr = _hyp_reference(prod, inner)
-    X, Y = tr["X"], tr["Y"]
-    s_of = torch.arange(B * im, device=DEV).repeat_interleave(ir)
-
-    def kabsch_of(inn):
-        Xk, Yk = X[s_of[:, None], inn], Y[s_of[:, None], inn]
-        Rr, tr_ = mo.kabsch(Xk, Yk)
-        Hm = (Xk - Xk.mean(1, keepdim=True)).transpose(1, 2) @ (Yk - Yk.mean(1, keepdim=True))
-        sv = torch.linalg.svdvals(Hm)
-        return Rr.reshape(-1, 9), tr_.reshape(-1, 3), sv[:, 1] > 1e-3 * sv[:, 0]
-
-    Rr, tr_, well = kabsch_of(inner)
-    well &= ~amb.reshape(-1)
-    assert float(well.float().mean()) > 0.5
-    got = prod.hyp_Rt.double()
-    bound_R, bound_t = 1e-3, 1e-3 * (1 + tr_.abs())
-
-    def misses(R_, t_):
-        return ((got[:, :9] - R_).abs().amax(1) > bound_R) | ((got[:, 9:] - t_).abs() > bound_t).any(1)
-
-    miss = misses(Rr, tr_) & well
-    assert int(miss.sum()) == 0, (prod.name, int(miss.sum()), int(well.sum()))
-    # power: one triple member replaced by its neighbour in the set
-    mut = inner.clone()
-    mut[:, 0] = (mut[:, 0] + 1) % N_S
-    Rm, tm, well_m = kabsch_of(mut)
-    rej = misses(Rm, tm)[well & well_m]
-    assert float(rej.float().mean()) > 0.9, float(rej.float().mean())
-    # soft inlier counts (the bound of test_solver_production_batch_injected_draws)
-    hyp, ref = prod.res["hyp_scores"].double(), tr["hyp_scores"].double()
-    wl = well.reshape(hyp.shape)
-    assert bool(((hyp - ref).abs() <= 1e-3 * ref.abs() + 1e-3)[wl].all())
-    # the pose: a tie-tolerant winner, and the oracle's pose where the winner is the same
-    win = hyp.argmax(1)
-    assert bool((ref.gather(1, win[:, None])[:, 0] >= ref.max(1).values * (1 - 1e-3)).all())
-    same = win == tr["best"]
-    if bool(same.any()):
-        assert float(rotation_angle_deg(prod.R[same].double(), Ro.reshape(B, 3, 3)[same]).max()) < 1e-2
-        assert float((prod.t.reshape(B, 3)[same].double() - to.reshape(B, 3)[same]).abs().max()) < 1e-3
-    print(f"\n[{prod.name}] {inner.shape[0]} hypotheses: {int(amb.sum())} ambiguous, {int(well.sum())} checked, "
-          f"neighbour mutation rejected in {float(rej.float().mean()):.4f}, same winner in {int(same.sum())}/{B} pairs")
+    stages.inner_draws_are_restated(prod)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -180,7 +98,7 @@ def test_layouts_of_the_production_matrix(prod):
     assert st_a == st_b == st_c == 0
     assert torch.equal(a, b) and torch.equal(a, c)
     for q in range(Bq):
-        _band_all(fs[q], b[q], q, IM, 99, f"{prod.name} layouts")
+        stages.band_all(fs[q], b[q], q, IM, 99, f"{prod.name} layouts")
 
 
 @pytest.mark.parametrize("N,IM", [(2500, 9),        # ROW_VEC with one row per 4096-cell chunk; a partial Philox group
@@ -195,7 +113,7 @@ def test_sizes(N, IM):
     buf[:, :, :N] = p
     idx, st = _sample(buf, pitch, IM, 1234)
     assert st == 0
-    d, n = _band_all(p[0], idx[0], 0, IM, 1234, f"N={N}")
+    d, n = stages.band_all(p[0], idx[0], 0, IM, 1234, f"N={N}")
     print(f"\n[N={N}] max cells differing {d}, in band {n}")
 
 
@@ -219,7 +137,7 @@ def test_edge_distributions(kind):
     p = _edge(kind, torch.Generator(device=DEV).manual_seed(7))
     idx, st = _sample(p, p.shape[-1], 16, 4321)
     assert st == 0
-    d, n = _band_all(p[0], idx[0], 0, 16, 4321, kind)
+    d, n = stages.band_all(p[0], idx[0], 0, 16, 4321, kind)
     if kind == "count2048":
         assert d == 0
     print(f"\n[{kind}] max cells differing {d}, in band {n}")
@@ -257,7 +175,7 @@ def test_failure_contract(case):
         elif case == "subnormal" and b == P:        # keys of subnormal p carry fewer bits than the band allows
             assert all(bool((pb[got[b, s]] > 0).all()) and got[b, s].unique().numel() == N_S for s in range(2))
         else:
-            _band_all(fsd[b], got[b], b, 2, SEED, case)
+            stages.band_all(fsd[b], got[b], b, 2, SEED, case)
     if case == "pos1":                              # ATen's fast path does not raise on CUDA either
         torch.multinomial(fsd[P].reshape(1, -1), N_S)
 
