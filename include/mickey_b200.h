@@ -197,6 +197,8 @@ long long mk_mutual_matches_ws_bytes(int B, int N);
  * scores sum to zero, so the inner torch.multinomial would raise.  Any of these bits gives the reference's zero result
  * (num_valid_h = 0).  A set with fewer than C positive scores is not a failure, as in torch: the positive entries are drawn
  * first and the entries that follow the last pick, cyclically, fill the rest.  Workspace: mk_loss_search_ws_bytes(B, IM).
+ * Sizes: S any multiple of 32 up to 2048 (64 and 512 in the reference's configs; the inlier masks are whole 32-bit words)
+ * and 1 <= C <= min(16, S), S <= N*N; anything else is MK_ERR_INVALID.
  *
  * mk_loss_gradient: probs_grad_dev fp32 [B, N, N] contiguous = mask_b (sum_i [cell in S_i] loss_i - count baseline_b) / IM
  * (:251-261, :299-316) from sampled_idx_dev int32 [B*IM, S] (any order), loss_value_dev fp32 [B*IM], baseline_dev fp32 [B]

@@ -49,7 +49,10 @@ loss_hyp_kernel(const int* __restrict__ idx, const float* __restrict__ fs, long 
   }
   if (tid == 0) { inv3x3(K0 + b * 9, Ki0); inv3x3(K1 + b * 9, Ki1); }
   __syncthreads();
-  const int per = S / LOSS_THREADS;
+  // gather_set's layout: thread t owns entries t * per + j < S, so at S < 256 (or S not a multiple of 256) the
+  // trailing threads own none and add 0 to the scan
+  const int per = (S + LOSS_THREADS - 1) / LOSS_THREADS;
+  const int own = min(per, max(S - tid * per, 0));
   float run;
   gather_set(idx, fs, kps0, d0, kps1, d1, Ki0, Ki1, N, pitch, b, s, S, LOSS_THREADS, X, Y, cdf, run);
   float inc = run;
@@ -62,7 +65,7 @@ loss_hyp_kernel(const int* __restrict__ idx, const float* __restrict__ fs, long 
   __syncthreads();
   float base = inc - run;
   for (int w = 0; w < warp; ++w) base += warp_tot[w];
-  for (int j = 0; j < per; ++j) cdf[tid * per + j] += base;
+  for (int j = 0; j < own; ++j) cdf[tid * per + j] += base;
   __syncthreads();
   const float W = cdf[S - 1];
   // torch.multinomial raises on a row that sums to zero (:159; the reference's try/except then zeroes the batch)
@@ -250,12 +253,13 @@ int loss_search(const float* fs, long long pitch, const float* kps0, const float
                 uint32_t* inl_out, int* status, void* ws, long long ws_bytes, cudaStream_t st) {
   if (pitch <= 0) pitch = N;
   if (!fs || !kps0 || !d0 || !kps1 || !d1 || !K0 || !K1 || !sampled_out || !inner_out || !inl_out || !status || !ws || B <= 0 ||
-      N <= 0 || pitch < N || IM <= 0 || IR <= 0 || n_ref < 0 || S <= 0 || S % LOSS_THREADS || S > LOSS_MAX_S || C < 1 ||
+      N <= 0 || pitch < N || IM <= 0 || IR <= 0 || n_ref < 0 || S <= 0 || S % 32 || S > LOSS_MAX_S || C < 1 ||
       C > LOSS_MAX_C || C > S || (long long)N * N < S || (long long)N * N > 0x7fffffffLL || !(th_ref == th_ref)) {
+    // S % 32: the inlier masks are whole 32-bit words, one bit per set entry
     set_last_error("mk_loss_search: need non-NULL inputs, outputs, status and workspace, B, N, IM, IR > 0, pitch >= N, "
-                   "n_ref >= 0, S a multiple of %d up to %d and <= N*N, 1 <= C <= min(%d, S), N*N < 2^31 and th_ref not NaN "
-                   "(got B %d N %d pitch %lld IM %d IR %d S %d C %d n_ref %d)", LOSS_THREADS, LOSS_MAX_S, LOSS_MAX_C, B, N,
-                   pitch, IM, IR, S, C, n_ref);
+                   "n_ref >= 0, S a multiple of 32 up to %d and <= N*N, 1 <= C <= min(%d, S), N*N < 2^31 and th_ref not NaN "
+                   "(got B %d N %d pitch %lld IM %d IR %d S %d C %d n_ref %d)", LOSS_MAX_S, LOSS_MAX_C, B, N, pitch, IM, IR,
+                   S, C, n_ref);
     return MK_ERR_INVALID;
   }
   if (ws_bytes < loss_search_ws_bytes(B, IM)) {

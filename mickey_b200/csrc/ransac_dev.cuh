@@ -36,23 +36,26 @@ __device__ __forceinline__ void inv3x3(const float* K, float* Ki) {
 }
 
 // Back-projected 3D points of one set of sampled matches, straight into the block's shared memory (X[3][n_s], Y[3][n_s])
-// together with the per-thread inclusive running sums of the match weights (cdf, when wanted): thread t owns the samples
-// t * per .. t * per + per - 1 (the order the weights' prefix sums are defined in).
+// together with the per-thread inclusive running sums of the match weights (cdf, when wanted): with
+// per = ceil(n_s / n_threads), thread t owns the samples t * per + j (j < per) that are < n_s (the order the weights'
+// prefix sums are defined in); threads past the end own none and keep run = 0.  When n_threads divides n_s this is
+// the plain split t * per .. t * per + per - 1.
 __device__ __forceinline__ void gather_set(const int* __restrict__ idx, const float* __restrict__ fs,
                                            const float* __restrict__ kps0, const float* __restrict__ d0,
                                            const float* __restrict__ kps1, const float* __restrict__ d1,
                                            const float* Ki0, const float* Ki1, int N, long long pitch, int b, long long s, int n_s,
                                            int n_threads, float* X, float* Y, float* cdf, float& run) {
-  const int per = n_s / n_threads;
+  const int per = (n_s + n_threads - 1) / n_threads;
+  const int own = min(per, max(n_s - (int)threadIdx.x * per, 0));          // samples this thread owns
   run = 0.f;
   // groups of 8 samples: the index -> keypoint / depth / score loads of a group are independent and issued together (the
   // score is a random access into the N x N matrix: one DRAM round trip per GROUP, not per sample); the running sum follows
-  for (int j0 = 0; j0 < per; j0 += 8) {
+  for (int j0 = 0; j0 < own; j0 += 8) {
     float wv[8];
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
       wv[jj] = 0.f;
-      if (j0 + jj < per) {
+      if (j0 + jj < own) {
         const int i = threadIdx.x * per + j0 + jj;
         const int cell = idx[s * n_s + i];
         const int i0 = cell / N, i1 = cell - i0 * N;
@@ -70,7 +73,7 @@ __device__ __forceinline__ void gather_set(const int* __restrict__ idx, const fl
     if (cdf) {
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj)
-        if (j0 + jj < per) { run += wv[jj]; cdf[threadIdx.x * per + j0 + jj] = run; }
+        if (j0 + jj < own) { run += wv[jj]; cdf[threadIdx.x * per + j0 + jj] = run; }
     }
   }
 }

@@ -28,6 +28,7 @@ from . import _lib
 
 STATUS_PRECHECK, STATUS_INNER = 16, 32          # include/mickey_b200.h MK_LOSS_STATUS_*
 STATUS_SKIP = 1 | 2 | STATUS_PRECHECK | STATUS_INNER
+LOSS_MAX_S, LOSS_MAX_C = 2048, 16              # csrc/ops.h: largest NUM_SAMPLES_MATCHES and NUM_CORR_3d3d
 
 
 def _stream(dev):
@@ -147,6 +148,13 @@ class LossParams:
         cl = lc.CURRICULUM_LEARNING
         self.train_w_top = bool(cl.TRAIN_WITH_TOPK or cl.TRAIN_CURRICULUM)
         self.topK = cl.TOPK_INIT if cl.TRAIN_CURRICULUM else (cl.TOPK if cl.TRAIN_WITH_TOPK else None)
+        # mk_loss_search's limits, checked here so that an unsupported config fails at construction, not at the first
+        # forward: the inlier masks are 32-bit words, one bit per set entry
+        if not (0 < self.n_sample <= LOSS_MAX_S and self.n_sample % 32 == 0):
+            raise ValueError(f"SAMPLER.NUM_SAMPLES_MATCHES must be a multiple of 32 up to {LOSS_MAX_S}, got {self.n_sample}")
+        if not (1 <= self.num_corr <= min(LOSS_MAX_C, self.n_sample)):
+            raise ValueError(f"GENERATE_HYPOTHESES.NUM_CORR_3d3d must be in [1, {LOSS_MAX_C}] and <= NUM_SAMPLES_MATCHES, "
+                             f"got {self.num_corr}")
 
 
 def loss_search(fs, kps0, d0, kps1, d1, K0, K1, p: LossParams, seed: int, outer_idx=None, inner_idx=None):
@@ -164,7 +172,7 @@ def loss_search(fs, kps0, d0, kps1, d1, K0, K1, p: LossParams, seed: int, outer_
     lib = _lib.load()
     sampled = torch.empty(B * IM, S, dtype=torch.int32, device=dev)
     inner = torch.empty(B * IM * IR, Cn, dtype=torch.int32, device=dev)
-    bits = torch.empty(B * IM * IR, S // 32 if S % 32 == 0 else 1, dtype=torch.int32, device=dev)
+    bits = torch.empty(B * IM * IR, S // 32, dtype=torch.int32, device=dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
     ws_bytes = int(lib.mk_loss_search_ws_bytes(B, IM))
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)

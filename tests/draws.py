@@ -26,6 +26,11 @@ kernel is deterministic, so `inner_cdf` and `inner_draw` restate it bit for bit 
 summation order, the uniforms of Philox(seed ^ 0x9E3779B97F4A7C15)(h, s_in, b, 0x3c6ef372), the removal of the drawn
 mass, the skip over drawn entries, the clamp below W and the guard.  `law3` is the closed-form law of successive
 sampling.
+
+The training loss (loss.cu, loss_hyp_kernel) draws C of its S set entries the same way, generalised: `loss_inner_cdf`
+is the cdf of its thread layout (S a multiple of 32, thread t owns entries t * ceil(S / 256) + j < S), and
+`loss_inner_draw` its C draws, with key seed ^ 0x9E3779B97F4A7C15, counters (h, s_in, b, 0xA54FF53A + k / 4) and the four
+words of one Philox call used by draws 4 (k / 4) .. 4 (k / 4) + 3.
 """
 import itertools
 import math
@@ -37,7 +42,9 @@ PHILOX_M0, PHILOX_M1 = 0xD2511F53, 0xCD9E8D57
 PHILOX_W0, PHILOX_W1 = 0x9E3779B9, 0xBB67AE85
 TAG_PREFIX, TAG_LOW = 0x5BD1E995, 0x2545F491
 INNER_SEED_XOR, INNER_TAG = 0x9E3779B97F4A7C15, 0x3C6EF372
+LOSS_INNER_TAG = 0xA54FF53A                      # loss.cu: 4th Philox counter of the loss's inner draw, + k / 4
 HYP_THREADS = 256                                # ransac_solve_kernel's block: the cdf is scanned across these threads
+LOSS_THREADS = 256                               # loss_hyp_kernel's block
 BAND = 1e-4                                      # relative key band around k* (module docstring)
 F32_ONE_MINUS_ULP = 1.0 - 2.0 ** -24             # 0.99999994f
 
@@ -144,16 +151,41 @@ def inner_cdf(w: torch.Tensor) -> torch.Tensor:
     for j in range(per):
         run = run + wv[:, :, j]
         loc[:, :, j] = run
-    t = torch.arange(HYP_THREADS, device=w.device)
+    return (loc + _scan_base(run)[:, :, None]).reshape(S, n)
+
+
+def _scan_base(run: torch.Tensor) -> torch.Tensor:
+    """The exclusive base of every thread's run total [S, threads]: a shfl_up warp scan, inc - run, then the totals of
+    the preceding warps added one by one in warp order."""
+    threads = run.shape[1]
+    t = torch.arange(threads, device=run.device)
     lane, warp = t % 32, t // 32
     inc = run.clone()
     for o in (1, 2, 4, 8, 16):
         inc = torch.where(lane >= o, inc + torch.roll(inc, o, dims=1), inc)
-    wtot = inc.reshape(S, HYP_THREADS // 32, 32)[:, :, 31]
+    wtot = inc.reshape(run.shape[0], threads // 32, 32)[:, :, 31]
     base = inc - run
-    for wi in range(HYP_THREADS // 32 - 1):
+    for wi in range(threads // 32 - 1):
         base = torch.where(warp > wi, base + wtot[:, wi:wi + 1], base)
-    return (loc + base[:, :, None]).reshape(S, n)
+    return base
+
+
+def loss_inner_cdf(w: torch.Tensor) -> torch.Tensor:
+    """fp32 [R, S] weights -> loss_hyp_kernel's fp32 cdf [R, S] for any S that is a multiple of 32: with per =
+    ceil(S / 256), thread t adds the weights of entries t * per + j < S serially (a thread past the end owns none and its
+    total is 0), then the block scan of inner_cdf.  When 256 divides S this is inner_cdf's layout exactly; otherwise it
+    equals inner_cdf of the weights padded with zeros to 256 * per entries (adding an exact 0 changes no sum)."""
+    R, n = w.shape
+    per = -(-n // LOSS_THREADS)
+    pos = torch.arange(LOSS_THREADS, device=w.device)[:, None] * per + torch.arange(per, device=w.device)   # [256, per]
+    own = pos < n
+    wv = torch.where(own, w.float()[:, pos.clamp_max(n - 1)], torch.zeros((), device=w.device))             # [R, 256, per]
+    run = torch.zeros(R, LOSS_THREADS, dtype=torch.float32, device=w.device)
+    loc = torch.empty_like(wv)
+    for j in range(per):
+        run = torch.where(own[:, j], run + wv[:, :, j], run)
+        loc[:, :, j] = run
+    return (loc + _scan_base(run)[:, :, None]).reshape(R, LOSS_THREADS * per)[:, :n]
 
 
 def _ulp(x: torch.Tensor) -> torch.Tensor:
@@ -217,6 +249,75 @@ def inner_draw(cdf: torch.Tensor, seed: int, b_of: torch.Tensor, s_in_of: torch.
         ids.append(pick)
         removed = removed + entry(pick)[1]
     return torch.stack(ids, 1).reshape(S, IR, 3), amb.reshape(S, IR)
+
+
+def loss_inner_draw(cdf: torch.Tensor, seed: int, b_of: torch.Tensor, s_in_of: torch.Tensor, IR: int, C: int,
+                    ulps: int = 2, tag: int = LOSS_INNER_TAG, skip_in_draw_order: bool = False):
+    """The training loss's C-of-n draw (loss_hyp_kernel) for hypotheses 0 .. IR-1 of every set (row of cdf, from
+    loss_inner_cdf).  Draw k uses word k % 4 of Philox(seed ^ 0x9E3779B97F4A7C15)(h, s_in, b, tag + k / 4); its target
+    u (W - removed) skips the mass of the entries drawn so far in ascending index order, is clamped to W (1 - 2^-24), and
+    the first cdf entry above it is taken; the guard then advances a pick that was already drawn, cyclically, up to C
+    times.  Returns (idx int64 [R, IR, C] in draw order, ambiguous bool [R, IR], as in inner_draw).  `tag` and
+    `skip_in_draw_order` exist to plant mutations."""
+    R, n = cdf.shape
+    dev = cdf.device
+    flat = cdf.reshape(-1)
+    h = torch.arange(IR, dtype=torch.int64, device=dev)
+    words = []
+    for q in range(-(-C // 4)):
+        r = philox(h[None, :], s_in_of[:, None].to(dev), b_of[:, None].to(dev), tag + q, seed ^ INNER_SEED_XOR)
+        words += [x.reshape(-1) for x in r]
+    row = (torch.arange(R, device=dev) * n).repeat_interleave(IR)
+
+    def at(i):
+        return flat[row + i]
+
+    def entry(i):
+        hi = at(i)
+        return hi, hi - torch.where(i > 0, at((i - 1).clamp_min(0)), torch.zeros_like(hi))
+
+    def near(a, b_):
+        return (a - b_).abs() <= ulps * torch.maximum(_ulp(a), _ulp(b_))
+
+    W = at(torch.full_like(row, n - 1))
+    clampW = W * torch.tensor(F32_ONE_MINUS_ULP, dtype=torch.float32, device=dev)
+    removed = torch.zeros_like(W)
+    amb = torch.zeros(R * IR, dtype=torch.bool, device=dev)
+    ids = []
+    for k in range(C):
+        u = ((words[k] >> 8).float() + 0.5) * 2.0 ** -24                               # u01_from_bits, in fp32
+        target = u * (W - removed)
+        if k > 0:
+            prev = torch.stack(ids, 1)
+            for x in (prev if skip_in_draw_order else prev.sort(1).values).unbind(1):
+                hi, ex = entry(x)
+                edge = hi - ex
+                amb |= near(target, edge)
+                target = torch.where(target >= edge, target + ex, target)
+        tq = torch.minimum(target, clampW)
+        lo = torch.zeros_like(row)
+        hi_i = torch.full_like(row, n - 1)
+        for _ in range(math.ceil(math.log2(n)) + 1):
+            act = lo < hi_i
+            mid = (lo + hi_i) >> 1
+            right = at(mid) > tq
+            hi_i = torch.where(act & right, mid, hi_i)
+            lo = torch.where(act & ~right, mid + 1, lo)
+        pick = lo
+        amb |= near(tq, at(pick)) | ((pick > 0) & near(tq, at((pick - 1).clamp_min(0))))
+        if k > 0:
+            for _ in range(C):                                                          # the guard
+                pick = torch.where((prev == pick[:, None]).any(1), (pick + 1) % n, pick)
+        ids.append(pick)
+        removed = removed + entry(pick)[1]
+    return torch.stack(ids, 1).reshape(R, IR, C), amb.reshape(R, IR)
+
+
+def inner_draw_check(got: torch.Tensor, want: torch.Tensor, amb: torch.Tensor) -> dict:
+    """Kernel inner draws [R, IR, C] against loss_inner_draw's: `ok` when every hypothesis that differs is ambiguous."""
+    diff = (got.to(want.device, torch.int64) != want).any(-1)
+    bad = diff & ~amb
+    return {"ok": int(bad.sum()) == 0, "n_bad": int(bad.sum()), "n_diff": int(diff.sum()), "n_amb": int(amb.sum())}
 
 
 # ---------------------------------------------------------------------------------------------------------------

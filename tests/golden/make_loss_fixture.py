@@ -14,6 +14,11 @@
     kps0_grad, kps1_grad, depth0_grad, depth1_grad            after avg_loss.backward()
     num_valid_h, mask_topk, avg_loss_rot, avg_loss_trans
   "vcre_grid" float64 [196, 3]: the reference's eye_coords_glob[:, :3] (lib/benchmarks/reprojection.py:32-60).
+
+    MICKEY_REFERENCE_ROOT=<reference checkout> python tests/golden/make_loss_fixture.py --warm-up
+
+  reference_loss_warmup_small.npz, the same keys for every case of tests/loss_cases.py WARMUP_CASES: the reference's two
+  warm-up configs (64 samples per set, no null hypothesis; top-K at B = 4 in the curriculum one), VCRE and POSE_ERR.
 The reference runs on the CPU in float32, as written.
 """
 import contextlib
@@ -87,11 +92,11 @@ def recording(lc):
         torch.multinomial, lc.weighted_procrustes, lc.soft_inlier_counting_3d = mult, wp, sc
 
 
-def record():
+def record(cases=loss_cases.CASES, seed0=1000):
     lc, rp = reference_loss_module()
     out = {"vcre_grid": np.asarray(rp.eye_coords_glob[:, :3], dtype=np.float64)}
-    for i, name in enumerate(loss_cases.CASES):
-        torch.manual_seed(1000 + i)
+    for i, name in enumerate(cases):
+        torch.manual_seed(seed0 + i)
         batch = loss_cases.case_batch(name)
         loss = lc.MetricPoseLoss(loss_cases.case_cfg(name))
         with recording(lc) as rec:
@@ -127,5 +132,9 @@ def record():
 
 
 if __name__ == "__main__":
-    np.savez_compressed(loss_cases.FIXTURE, **record())
-    print("wrote", loss_cases.FIXTURE, os.path.getsize(loss_cases.FIXTURE), "bytes")
+    if "--warm-up" in sys.argv[1:]:
+        path, rec = loss_cases.WARMUP_FIXTURE, record(loss_cases.WARMUP_CASES, 2000)
+    else:
+        path, rec = loss_cases.FIXTURE, record()
+    np.savez_compressed(path, **rec)
+    print("wrote", path, os.path.getsize(path), "bytes")

@@ -101,7 +101,8 @@ def reference_cfgs():
     _swap_lib(REF)
     from config.default import cfg as ref_cfg
     out = {}
-    for f in ("curriculum_learning.yaml", "overlap_score.yaml"):
+    for f in ("curriculum_learning.yaml", "overlap_score.yaml", "curriculum_learning_warm_up.yaml",
+              "overlap_score_warm_up.yaml"):
         c = ref_cfg.clone()
         c.merge_from_file(os.path.join(REF, "config", "MicKey", f))
         out[f] = c.dump()

@@ -30,6 +30,37 @@ CASES = {
 }
 
 
+WARMUP_FIXTURE = os.path.join(GOLDEN, "reference_loss_warmup_small.npz")
+# The reference's warm-up configs (64 samples per set, no null hypothesis; top-K from 30 % in the curriculum one, none in
+# the overlap-score one), as they are apart from the hypothesis budget.
+# case -> (golden features, pairs taken from it, reference config, LOSS_FUNCTION, SOFT_CLIPPING)
+WARMUP_CASES = {
+    "warm_curriculum_vits_topk_b4": ("vits_small", [0, 1, 1, 0], "curriculum_learning_warm_up", "VCRE", True),
+    "warm_curriculum_vitb_pose": ("vitb_small", [0, 0], "curriculum_learning_warm_up", "POSE_ERR", True),
+    "warm_overlap_vits_vcre": ("vits_small", [0, 1], "overlap_score_warm_up", "VCRE", True),
+    "warm_overlap_vitb_pose_hard": ("vitb_small", [0, 0], "overlap_score_warm_up", "POSE_ERR", False),
+}
+
+
+def reference_cfg(name, it_matches=None, it_ransac=None):
+    """The reference config tests/golden/reference_cfg_<name>.yaml, with the hypothesis budget replaced when given."""
+    cfg = default_cfg()
+    cfg.merge_from_file(os.path.join(GOLDEN, f"reference_cfg_{name}.yaml"))
+    g = cfg.LOSS_CLASS.GENERATE_HYPOTHESES
+    if it_matches is not None:
+        g.IT_MATCHES = it_matches
+    if it_ransac is not None:
+        g.IT_RANSAC = it_ransac
+    return cfg
+
+
+def warmup_cfg(name):
+    _, _, ref, loss, soft = WARMUP_CASES[name]
+    cfg = reference_cfg(ref, IM, IR)
+    cfg.LOSS_CLASS.LOSS_FUNCTION, cfg.LOSS_CLASS.SOFT_CLIPPING = loss, soft
+    return cfg
+
+
 def loss_cfg(loss="VCRE", soft=True, null=True, topk=False, it_matches=IM, it_ransac=IR):
     cfg = default_cfg()
     cfg.merge_from_file(os.path.join(GOLDEN, "reference_cfg_curriculum_learning.yaml"))
@@ -43,6 +74,8 @@ def loss_cfg(loss="VCRE", soft=True, null=True, topk=False, it_matches=IM, it_ra
 
 
 def case_cfg(name):
+    if name in WARMUP_CASES:
+        return warmup_cfg(name)
     _, _, loss, soft, null, topk = CASES[name]
     return loss_cfg(loss, soft, null, topk)
 
@@ -92,7 +125,7 @@ def plant(fs, kps0, kps1, seed=0, K=None):
 
 
 def case_batch(name):
-    src, pairs, *_ = CASES[name]
+    src, pairs, *_ = CASES[name] if name in CASES else WARMUP_CASES[name]
     z = np.load(os.path.join(GOLDEN, f"{src}.npz"))
     take = lambda k: torch.from_numpy(z[k][pairs])
     return plant(take("final_scores"), take("kps0"), take("kps1"), seed=len(pairs))

@@ -99,6 +99,82 @@ def test_inner_draw_takes_positive_entries_and_follows_the_guard():
     assert bool((idx[1] == torch.tensor([2047, 0, 1])).all())
 
 
+@pytest.mark.parametrize("n", [32, 64, 96, 256, 288, 512, 2048])
+def test_loss_inner_cdf_layout(n):
+    """The loss kernel's cdf: inner_cdf's exactly when 256 divides the set size; for any other multiple of 32, inner_cdf
+    of the weights padded with exact zeros to a multiple of 256 (the trailing threads add nothing).  On weights that
+    span 12 decades it is not a plain cumulative sum."""
+    g = torch.Generator().manual_seed(n)
+    w = (10.0 ** (-12 * torch.rand(6, n, generator=g))).float()
+    w[0, ::3] = 0
+    cdf = draws.loss_inner_cdf(w)
+    assert cdf.shape == (6, n)
+    per = -(-n // 256)
+    padded = torch.cat([w, torch.zeros(6, 256 * per - n)], 1)
+    assert torch.equal(cdf, draws.inner_cdf(padded)[:, :n])
+    if n % 256 == 0:
+        assert torch.equal(cdf, draws.inner_cdf(w))
+    assert not torch.equal(cdf, torch.cumsum(w.double(), 1).float())
+    wi = torch.randint(0, 5, (3, n), generator=g).float()
+    assert torch.equal(draws.loss_inner_cdf(wi), torch.cumsum(wi, 1))
+
+
+def _loss_sets(n, rows=16, seed=4):
+    """Set weights as the loss sees them: final_scores-like values over four decades, a few exact zeros."""
+    g = torch.Generator().manual_seed(seed)
+    w = (10.0 ** (-4 * torch.rand(rows, n, generator=g))).float()
+    w[torch.rand(rows, n, generator=g) < 0.1] = 0
+    return w, torch.arange(rows) // 4, torch.arange(rows) % 4
+
+
+def test_loss_inner_draw_at_three_with_the_solver_tag_is_the_solver_draw():
+    """The C-draw restatement with C = 3 and the solver's Philox tag is the solver's restated draw, element for element
+    (the two kernels share the cdf search, the skip and the guard)."""
+    w, b_of, s_in = _loss_sets(512)
+    cdf = draws.loss_inner_cdf(w)
+    got, amb = draws.loss_inner_draw(cdf, 0xC0FFEE, b_of, s_in, 40, 3, tag=draws.INNER_TAG)
+    want, amb3 = draws.inner_draw(draws.inner_cdf(w), 0xC0FFEE, b_of, s_in, 40)
+    assert torch.equal(got, want) and torch.equal(amb, amb3)
+
+
+def test_loss_inner_draw_check_rejects_planted_mutations():
+    """8 of 64: the check accepts the restatement itself and rejects the solver's tag in place of the loss's, one pick
+    replaced by its neighbour, and the skip over drawn mass taken in draw order instead of index order."""
+    n, C, IR, seed = 64, 8, 64, 0x5EED
+    w, b_of, s_in = _loss_sets(n)
+    cdf = draws.loss_inner_cdf(w)
+    want, amb = draws.loss_inner_draw(cdf, seed, b_of, s_in, IR, C)
+    assert bool((want.sort(-1).values[..., 1:] > want.sort(-1).values[..., :-1]).all())       # C distinct entries
+    assert draws.inner_draw_check(want, want, amb)["ok"]
+    assert int(amb.sum()) < amb.numel() // 10
+    tag, _ = draws.loss_inner_draw(cdf, seed, b_of, s_in, IR, C, tag=draws.INNER_TAG)
+    r = draws.inner_draw_check(tag, want, amb)
+    assert not r["ok"] and r["n_bad"] > amb.numel() // 2
+    clear = torch.nonzero(~amb)
+    nb = want.clone()
+    r0, h0 = int(clear[0, 0]), int(clear[0, 1])
+    nb[r0, h0, 5] = (nb[r0, h0, 5] + 1) % n
+    r = draws.inner_draw_check(nb, want, amb)
+    assert not r["ok"] and r["n_bad"] == 1
+    order, _ = draws.loss_inner_draw(cdf, seed, b_of, s_in, IR, C, skip_in_draw_order=True)
+    r = draws.inner_draw_check(order, want, amb)
+    assert not r["ok"] and r["n_bad"] >= 1
+
+
+def test_loss_inner_draw_fills_by_the_guard():
+    """5 positive weights of 64, 8 draws: the first five are the positive entries and the guard keeps the other three
+    distinct.  With one positive entry the draw is it and the seven entries after it, cyclically."""
+    n, C = 64, 8
+    w = torch.zeros(2, n)
+    pos = [3, 17, 40, 41, 63]
+    w[0, pos] = torch.tensor([1.0, 0.2, 0.05, 0.3, 1e-3])
+    w[1, 60] = 0.5
+    idx, _ = draws.loss_inner_draw(draws.loss_inner_cdf(w), 99, torch.tensor([0, 0]), torch.tensor([0, 1]), 200, C)
+    assert bool((idx[0, :, :5].sort(-1).values == torch.tensor(pos)).all())
+    assert bool((idx[0].sort(-1).values[:, 1:] > idx[0].sort(-1).values[:, :-1]).all())
+    assert bool((idx[1] == torch.tensor([60, 61, 62, 63, 0, 1, 2, 3])).all())
+
+
 def test_closed_form_law_matches_torch_multinomial():
     """Successive sampling's closed form against torch.multinomial(w, 3) and against the fp64 race top-3 of w / Exp(1)
     (what ATen's multinomial without replacement computes), by chi^2 over 400 k draws; the with-replacement law is
