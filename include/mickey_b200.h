@@ -224,6 +224,9 @@ int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream);
 
 /* Number of kernel launches issued by this library since the handle was created (for bench.py). */
 long long mk_launch_count(mk_handle* h);
+/* 1 when kernels are launched with programmatic dependent launch (the default), 0 under MICKEY_PDL=0.  The environment
+ * is read once per process, at the first launch or the first call of this function. */
+int mk_pdl_enabled(void);
 /* Per-kernel-class device timing: while enabled every launch issued by the stages is bracketed by CUDA
  * events on the launch stream; mk_profile_read synchronises and writes "<class> <scopes> <total ms>" lines. */
 int mk_profile_enable(mk_handle* h, int enable);

@@ -107,6 +107,7 @@ EXPORTS = {
     "mk_loss_gradient_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int]),
     "mk_pose_to_submission": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "mk_launch_count": (C.c_longlong, [C.c_void_p]),
+    "mk_pdl_enabled": (C.c_int, []),
     "mk_set_seed": (C.c_int, [C.c_void_p, C.c_ulonglong, C.c_void_p]),
     "mk_profile_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "mk_profile_read": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),

@@ -649,6 +649,8 @@ int mk_loss_gradient(const int* sampled_idx, const float* loss_value, const floa
 
 long long mk_launch_count(mk_handle* h) { return h ? h->launches : -1; }
 
+int mk_pdl_enabled(void) { return pdl_enabled() ? 1 : 0; }
+
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream) {
   if (!h) return MK_ERR_INVALID;
   return seed_set(h->seed_dev, seed, (cudaStream_t)stream);

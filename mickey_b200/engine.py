@@ -8,6 +8,7 @@ the position embedding (same torch call as the reference, dinov2.py:165-189) and
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 from typing import Dict, Optional
@@ -224,6 +225,54 @@ class Engine:
         self._graphs, self._slot = {}, {}
         self._copy_stream = None
         self._pairs_ws = None
+        # set when the engine takes new blocks on the caller's stream (weights, tables, workspace, buffer sets): that stream
+        # may still have work queued on those blocks (writes of the weights and tables, or pending kernels of tensors freed
+        # there), so the streams that use them next wait on it once
+        self._caller_pending = False
+        self._last_ent = None           # buffer set of the last forward() call (release())
+
+    # -- streams -----------------------------------------------------------------------------------------------
+    # Engine buffers (packed weights, per-geometry tables, workspaces, the static buffer sets) are allocated on the
+    # caller's stream.  When the engine has a side stream they are also used there, so each one is passed to
+    # record_stream for it: when a buffer is dropped (batch growth, geometry eviction, weight reload) the caching
+    # allocator hands its block out again only after the side stream's work queued so far has finished.
+    def _own(self, t):
+        if t is not None and self.stream is not None:
+            t.record_stream(self.stream)
+        return t
+
+    def _buffers(self):
+        yield from self.packed.values()
+        yield self.ws
+        yield self._pairs_ws
+        for gs in self._geo_state.values():
+            yield from (gs[n] for n in ("patch.posb", "patch.clspos", "head.pe", "ws"))
+        for ent in self._graphs.values():
+            yield from ent["st"].values()
+
+    def use_side_stream(self):
+        """Give the engine its own stream from now on (MickeyRelativePose.pipeline_depth > 1).  Buffers allocated
+        before, and the graphs captured on the caller's stream, stay valid: the buffers are recorded for the new stream."""
+        if self.stream is None:
+            self.stream = torch.cuda.Stream(device=self.device)
+            for t in self._buffers():
+                self._own(t)
+            self._caller_pending = True
+
+    @contextlib.contextmanager
+    def _ordered(self):
+        """Handle calls outside forward() (the staged stages, feature banks, solve) run on the caller's stream.  They
+        share the handle's device RNG word and forward()'s workspace with the graph replays queued on the side stream,
+        so they run after that stream's queued work, and the side stream's later work runs after them."""
+        if self.stream is None:
+            yield
+            return
+        caller = torch.cuda.current_stream()
+        caller.wait_stream(self.stream)
+        try:
+            yield
+        finally:
+            self.stream.wait_stream(caller)
 
     def __del__(self):
         try:
@@ -246,7 +295,8 @@ class Engine:
                                  sd[BACKBONE + "cls_token"].detach().to(self.device).float(),
                                  sd[BACKBONE + "patch_embed.proj.bias"].detach().to(self.device).float())
         for name, t in self.packed.items():
-            self._register(name, t)
+            self._register(name, self._own(t))
+        self._caller_pending = True
         # captured graphs hold raw pointers of the previous packed weights and tables: none of them may be replayed
         self._graphs.clear()
         self._slot.clear()
@@ -265,8 +315,9 @@ class Engine:
         self._use_geometry(H, W)
         if self.ws is None or self.ws_pairs < n_pairs:
             nbytes = self.lib.mk_workspace_bytes(self.h, n_pairs, H, W)
-            self.ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            self.ws = self._own(torch.empty(nbytes, dtype=torch.uint8, device=self.device))
             self.ws_pairs = n_pairs
+            self._caller_pending = True
         return self.ws
 
     def _use_geometry(self, H: int, W: int):
@@ -284,6 +335,9 @@ class Engine:
                     gs = {"patch.posb": (full[1:] + pbias[None]).contiguous(),
                           "patch.clspos": (cls.reshape(-1) + full[0]).contiguous(),
                           "head.pe": sine_table_padded(gh, gw).to(self.device), "ws": None, "ws_pairs": 0}
+                for n in ("patch.posb", "patch.clspos", "head.pe"):
+                    self._own(gs[n])
+                self._caller_pending = True
                 if len(self._geo_state) >= self.MAX_GEOMETRIES:      # evict the oldest geometry together with its graphs
                     old = next(iter(self._geo_state))
                     del self._geo_state[old]
@@ -338,7 +392,8 @@ class Engine:
         if self.ws_pairs != n_pairs:
             nbytes = self.lib.mk_workspace_bytes(self.h, n_pairs, H, W)
             if self.ws.numel() < nbytes:
-                self.ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+                self.ws = self._own(torch.empty(nbytes, dtype=torch.uint8, device=self.device))
+                self._caller_pending = True
             self.ws_pairs = n_pairs
         return self.ws
 
@@ -375,8 +430,9 @@ class Engine:
         ws = self._ws_for(B, H, W)
         kps, depth, scr, dsc = self._outputs_of_extract(n_img, N)
         fn = self.lib.mk_extract_u8 if u8 else self.lib.mk_extract
-        _lib.check(fn(self.h, _lib.ptr(images), B, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
-                      _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), self._stream()), "mk_extract")
+        with self._ordered():
+            _lib.check(fn(self.h, _lib.ptr(images), B, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
+                          _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), self._stream()), "mk_extract")
         return kps, depth, scr, dsc
 
     # -- feature banks: extract images once, then match / solve any pairs among them ------------------------------
@@ -400,8 +456,9 @@ class Engine:
         ws = self._bank_ws(n_img, 0, H, W)
         kps, depth, scr, dsc = self._outputs_of_extract(n_img, N)
         fn = self.lib.mk_extract_images_u8 if u8 else self.lib.mk_extract_images
-        _lib.check(fn(self.h, _lib.ptr(images), n_img, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
-                      _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), self._stream()), "mk_extract_images")
+        with self._ordered():
+            _lib.check(fn(self.h, _lib.ptr(images), n_img, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
+                          _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), self._stream()), "mk_extract_images")
         return kps, depth, scr, dsc
 
     def forward_pairs(self, bank0, idx0, bank1, idx1, K0, K1, seed: int, image_size, lean: bool = False):
@@ -426,11 +483,12 @@ class Engine:
         K1 = K1.to(dev, torch.float32).contiguous()
         seed = (int(seed) & (2 ** 64 - 1)) or 1
         p = _lib.ptr
-        _lib.check(self.lib.mk_forward_pairs(
-            self.h, *(p(t) for t in bank0), bank0[0].shape[0], *(p(t) for t in bank1), bank1[0].shape[0], p(idx0), p(idx1),
-            p(K0), p(K1), P, C.c_ulonglong(seed), p(out["kps"]), p(out["depth"]), p(out["scores"]), p(out["kp_scores"]),
-            p(out["final_scores"]), out["final_scores"].stride(1), p(out["pose"]), p(out["best_set"]), p(out["inlier_mask"]),
-            p(out["sampled_idx"]), p(out["status"]), p(ws), ws.numel(), self._stream()), "mk_forward_pairs")
+        with self._ordered():
+            _lib.check(self.lib.mk_forward_pairs(
+                self.h, *(p(t) for t in bank0), bank0[0].shape[0], *(p(t) for t in bank1), bank1[0].shape[0], p(idx0), p(idx1),
+                p(K0), p(K1), P, C.c_ulonglong(seed), p(out["kps"]), p(out["depth"]), p(out["scores"]), p(out["kp_scores"]),
+                p(out["final_scores"]), out["final_scores"].stride(1), p(out["pose"]), p(out["best_set"]), p(out["inlier_mask"]),
+                p(out["sampled_idx"]), p(out["status"]), p(ws), ws.numel(), self._stream()), "mk_forward_pairs")
         return out
 
     def match(self, B: int, N: int, lean: bool = False):
@@ -439,8 +497,9 @@ class Engine:
         scores = None if lean else nn_empty(B, N, dev)
         kp_scores = None if lean else nn_empty(B, N, dev)
         final = nn_empty(B, N, dev)
-        _lib.check(self.lib.mk_match(self.h, B, _lib.ptr(scores), _lib.ptr(kp_scores), _lib.ptr(final), final.stride(1),
-                                     _lib.ptr(self.ws), self.ws.numel(), self._stream()), "mk_match")
+        with self._ordered():
+            _lib.check(self.lib.mk_match(self.h, B, _lib.ptr(scores), _lib.ptr(kp_scores), _lib.ptr(final), final.stride(1),
+                                         _lib.ptr(self.ws), self.ws.numel(), self._stream()), "mk_match")
         return scores, kp_scores, final
 
     # -- whole path in one C call, optionally replayed from a CUDA graph -------------------------------------------
@@ -473,9 +532,15 @@ class Engine:
         """Whole hot path (extract -> match -> solve) for a batch of pairs.
 
         Returns the dict of STATIC output tensors of this (B, H, W) geometry.  Two buffer sets alternate, so the
-        tensors of one call stay valid until the call after the next one with the same geometry.  Host (pinned)
+        tensors of one call stay valid until the call after the next one with the same geometry on this engine.  That
+        window is in stream order when this engine's work waits on the caller's stream (no side stream, or device
+        inputs without assume_inputs_ready), or for reads the caller announced with release().  Otherwise it holds in
+        host order only: reads of a call's outputs queued on the caller's stream must have completed (synchronise that
+        stream) before the call that reuses the buffer set is issued; waiting on the caller's stream instead would
+        serialise the pipeline, since the caller waits on every call's completion.  Host (pinned)
         inputs are copied H2D on a side stream into the other buffer set while the previous call is still
-        computing; device inputs are copied D2D on the main stream."""
+        computing; device inputs are copied D2D on the main stream, after the caller's stream has produced them
+        (unless assume_inputs_ready).  Inputs of another floating dtype (fp64 K, say) are converted by those copies."""
         B = image0.shape[0]
         u8 = image0.dtype == torch.uint8                 # [B, H, W, 3] RGB straight from the decoder (mk_forward_u8)
         if u8:
@@ -496,36 +561,60 @@ class Engine:
         key = (B, H, W, slot, fmt)
         ent = self._graphs.get(key)
         if ent is None or ent["ws_ptr"] != self.ws.data_ptr():
-            ent = {"st": self._static_buffers(B, H, W, u8, lean), "graph": None, "launches": 0, "ws_ptr": self.ws.data_ptr(),
-                   "calls": 0, "done": None}
+            ent = {"st": {k: self._own(t) for k, t in self._static_buffers(B, H, W, u8, lean).items()}, "graph": None,
+                   "launches": 0, "ws_ptr": self.ws.data_ptr(), "calls": 0, "done": None, "readers": set()}
             self._graphs[key] = ent
+            self._caller_pending = True
         st = ent["st"]
         caller = torch.cuda.current_stream()
         main = self.stream if self.stream is not None else caller
-        if self.stream is not None and image0.device.type != "cpu" and not self.assume_inputs_ready:
-            main.wait_stream(caller)                    # device inputs may still be being produced on the caller's stream
+        ops = (image0, image1, K0, K1)
+        fresh, self._caller_pending = self._caller_pending, False
+        if self.stream is not None:
+            if ent.get("released") is not None:
+                main.wait_event(ent["released"])        # the caller's reads of this set's previous outputs
+                ent["released"] = None
+            if caller.cuda_stream not in ent["readers"]:
+                # the caller reads the outputs on its own stream: a dropped buffer set is reused only after that
+                ent["readers"].add(caller.cuda_stream)
+                for t in st.values():
+                    if t is not None:
+                        t.record_stream(caller)
+            on_device = any(t.device.type != "cpu" for t in ops)
+            if fresh or (on_device and not self.assume_inputs_ready):
+                main.wait_stream(caller)                # device inputs may still be being produced on the caller's stream
         with torch.cuda.stream(main):
-            self._forward_on(main, ent, st, image0, image1, K0, K1, B, H, W, seed, use_graph)
+            self._forward_on(main, ent, st, ops, B, H, W, seed, use_graph, caller if fresh else None)
         if self.stream is not None:
             caller.wait_event(ent["done"])              # outputs are safe to consume on the caller's stream
+        self._last_ent = ent
         return st
 
-    def _forward_on(self, main, ent, st, image0, image1, K0, K1, B, H, W, seed, use_graph):
-        if image0.device.type == "cpu":
+    def release(self):
+        """The caller's stream has queued every read of the outputs the last forward() returned.  The call that reuses
+        that buffer set waits for those reads (an event on the caller's stream), not for the caller's stream as a whole,
+        so steps stay in flight.  Without a side stream the caller's stream orders everything and this does nothing."""
+        if self.stream is not None and self._last_ent is not None:
+            ev = torch.cuda.Event()
+            ev.record()
+            self._last_ent["released"] = ev
+
+    def _forward_on(self, main, ent, st, ops, B, H, W, seed, use_graph, caller_pending):
+        dst = (st["images"][:B], st["images"][B:], st["K0"], st["K1"])
+        if any(t.device.type == "cpu" for t in ops):
             cs = self._copy_stream
+            if caller_pending is not None:
+                cs.wait_stream(caller_pending)          # new input buffers: blocks the caller's stream may still be using
             if ent["done"] is not None:
                 cs.wait_event(ent["done"])              # the graph that last read this input buffer has finished
             with torch.cuda.stream(cs):
-                st["images"][:B].copy_(image0, non_blocking=True)
-                st["images"][B:].copy_(image1, non_blocking=True)
-                st["K0"].copy_(K0, non_blocking=True)
-                st["K1"].copy_(K1, non_blocking=True)
+                for d, s in zip(dst, ops):
+                    if s.device.type == "cpu":
+                        d.copy_(s, non_blocking=True)
             main.wait_stream(cs)
-        else:
-            st["images"][:B].copy_(image0, non_blocking=True)
-            st["images"][B:].copy_(image1, non_blocking=True)
-            st["K0"].copy_(K0, non_blocking=True)
-            st["K1"].copy_(K1, non_blocking=True)
+        for d, s in zip(dst, ops):                      # device operands: in order behind the caller's stream (see forward)
+            if s.device.type != "cpu":
+                d.copy_(s, non_blocking=True)
         seed = (int(seed) & (2 ** 64 - 1)) or 1
         if not use_graph:
             self._call_forward(st, B, H, W, seed)
@@ -570,10 +659,11 @@ class Engine:
             inner_idx = inner_idx.to(dev, torch.int32).contiguous()
         K0 = K0.to(dev, torch.float32).contiguous()
         K1 = K1.to(dev, torch.float32).contiguous()
-        _lib.check(self.lib.mk_solve_pose(
-            self.h, _lib.ptr(final_scores), final_scores.stride(1), _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(K0), _lib.ptr(K1), B, N,
-            C.c_ulonglong(seed & (2 ** 64 - 1)), _lib.ptr(outer_idx), _lib.ptr(inner_idx), _lib.ptr(pose),
-            _lib.ptr(best_set), _lib.ptr(mask), _lib.ptr(sampled), _lib.ptr(hyp), _lib.ptr(status),
-            _lib.ptr(self.ws), self.ws.numel(), self._stream()), "mk_solve_pose")
+        with self._ordered():
+            _lib.check(self.lib.mk_solve_pose(
+                self.h, _lib.ptr(final_scores), final_scores.stride(1), _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(K0), _lib.ptr(K1), B, N,
+                C.c_ulonglong(seed & (2 ** 64 - 1)), _lib.ptr(outer_idx), _lib.ptr(inner_idx), _lib.ptr(pose),
+                _lib.ptr(best_set), _lib.ptr(mask), _lib.ptr(sampled), _lib.ptr(hyp), _lib.ptr(status),
+                _lib.ptr(self.ws), self.ws.numel(), self._stream()), "mk_solve_pose")
         return {"pose": pose, "status": status, "best_set": best_set, "inlier_mask": mask, "sampled_idx": sampled,
                 "hyp_scores": hyp}

@@ -321,8 +321,8 @@ class MickeyRelativePose(nn.Module):
                 e.load_state_dict(None, share_with=first)
                 pool.append(e)
             self.__dict__["_pool_version"] = self._eng_version
-        if depth > 1 and first.stream is None:
-            first.stream = torch.cuda.Stream(device=first.device)
+        if depth > 1:
+            first.use_side_stream()
         engines = [first] + pool
         for e in engines:
             e.assume_inputs_ready = bool(getattr(self, "assume_inputs_ready", False))
@@ -363,8 +363,10 @@ class MickeyRelativePose(nn.Module):
     @torch.no_grad()
     def forward(self, data, return_inliers=False):
         """One C call (mk_forward) per batch, replayed from a CUDA graph after the first two calls.
-        `self.static_outputs = True` hands out the engine's static output buffers directly (they are overwritten
-        by the next forward of the same geometry); the default clones them so that every call returns fresh
+        `self.static_outputs = True` hands out the engine's static output buffers directly (they are overwritten by the
+        forward after the next one of the same geometry on the same engine; with pipeline_depth > 1 under
+        assume_inputs_ready or with host inputs, reads of them must have completed before that call is issued, see
+        Engine.forward); the default clones them so that every call returns fresh
         tensors like the reference does.  `self.lean_outputs = True` skips data['scores'] / data['kp_scores'] (the solver
         only reads final_scores): 17 instead of 47 MB of N x N traffic per 720x540 pair."""
         if getattr(self, "staged", False):
@@ -376,9 +378,9 @@ class MickeyRelativePose(nn.Module):
         im0, im1 = data["image0"], data["image1"]
         B = im0.shape[0]
         seed = int(torch.randint(1, 2 ** 62, (1,)).item())
-        if im0.dtype != torch.uint8:                     # uint8 [B,H,W,3] goes to the ingest kernel as it is (mickey_b200.io)
-            im0, im1 = im0.float(), im1.float()
-        st = eng.forward(im0, im1, data["K_color0"].float(), data["K_color1"].float(), seed,
+        # uint8 [B,H,W,3] goes to the ingest kernel as it is (mickey_b200.io); other dtypes (fp64 K, say) are converted by
+        # the engine's copies into its fp32 input buffers, on the stream that also reads them
+        st = eng.forward(im0, im1, data["K_color0"], data["K_color1"], seed,
                          use_graph=getattr(self, "use_graph", True), lean=bool(getattr(self, "lean_outputs", False)))
         keep = (lambda t: t) if getattr(self, "static_outputs", False) else (lambda t: t.clone())
         H, W = eng.geo
@@ -398,6 +400,8 @@ class MickeyRelativePose(nn.Module):
         R, t, inliers = pose[:, :9].reshape(B, 3, 3), pose[:, 9:12].reshape(B, 1, 3), pose[:, 12:13]
         if return_inliers:
             data["inliers_list"] = self._inlier_list(data, st, B, N)
+        if not getattr(self, "static_outputs", False):
+            eng.release()                                # every read of the static buffers above is queued
         data["R"], data["t"], data["inliers"] = R, t, inliers
         return R, t
 
