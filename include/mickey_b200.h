@@ -218,6 +218,44 @@ int mk_loss_gradient(const int* sampled_idx_dev, const float* loss_value_dev, co
                      void* stream);
 long long mk_loss_gradient_ws_bytes(int B, int it_matches, int n_sample);
 
+/* ---- training: the dual-softmax matcher on the caller's descriptors and its backward (mickey_b200/dual_softmax.py wraps
+ * both as a torch.autograd.Function).  Replaces dualSoftmax.forward (feature_matcher.py:64-83), kp_matrix_scores
+ * (compute_correspondences.py:46-50) and scores * kp_scores (model.py:201), and autograd through them.  No handle.
+ *
+ * mk_dual_softmax: dsc0_dev / dsc1_dev fp32 [B, 128, N] channel-major (prepare_kpts_dsc's layout), scr0 / scr1 fp32 [B, N]
+ * (both or neither), dustbin_dev a device fp32 scalar (USE_DUSTBIN) or NULL, temperature T > 0, 2 <= N <= 8192.
+ * Writes scores, kp_scores and final_scores together (scr required), final_scores alone, or scores alone, fp32
+ * [B, N, N] with row pitch nn_pitch floats (N or 0 = contiguous; a multiple of 4 lets them leave through TMA as in
+ * mk_match); without scr, kp_scores = 1 and final_scores = scores.  lse_r_dev / lse_c_dev fp32 [B, npad] (npad = N
+ * rounded up to 128): the log2-domain log-sum-exps of every row / column, which the backward reads.  unit_norm = 1 when
+ * every descriptor has norm <= 1 (DSC_HEAD.NORM_DSC): it selects mk_match's fixed-shift row / column partials, and with
+ * it the outputs are bit-identical to mk_match on the same descriptors (mk_match under NORM_DSC True for unit_norm = 1,
+ * False for 0).  The descriptors enter the tensor cores as hi + lo fp16 pairs (as in mk_extract): |dsc| must stay below
+ * 65504, and each value is carried to about 2^-22 relative plus 2^-25 absolute.
+ *
+ * mk_dual_softmax_backward: the forward's inputs and its lse_r / lse_c, plus the gradients of the three outputs,
+ * grad_scores / grad_kp / grad_final fp32 [B, N, pitch] (pitch >= N floats, 0 = N; pairs N rows apart), any of which
+ * may be NULL but not all; grad_kp needs scr.  Out: ddsc0 / ddsc1 fp32 [B, 128, N], dscr0 / dscr1 fp32 [B, N] (required
+ * with scr, ignored without), ddustbin fp32 [1] (required with the dustbin; the sum over the batch).  The backward runs
+ * in fp32 on the CUDA cores and writes no N x N intermediate; it is deterministic, and a pair's ddsc / dscr are the same
+ * bits alone or inside a batch.
+ *
+ * Workspaces: mk_dual_softmax_ws_bytes(B, N) / mk_dual_softmax_backward_ws_bytes(B, N) bytes, 256-byte aligned (0 for
+ * unsupported sizes).  Bad arguments return MK_ERR_INVALID and launch nothing.  Both calls always use the wgmma and
+ * fp32 kernels; MICKEY_GEMM_IMPL does not apply to them.  Capturing them in a CUDA graph is not tested. */
+long long mk_dual_softmax_ws_bytes(int B, int N);
+long long mk_dual_softmax_backward_ws_bytes(int B, int N);
+int mk_dual_softmax(const float* dsc0_dev, const float* dsc1_dev, const float* scr0_dev, const float* scr1_dev,
+                    const float* dustbin_dev, float temperature, int B, int N, int unit_norm, float* scores_dev,
+                    float* kp_scores_dev, float* final_scores_dev, long long nn_pitch, float* lse_r_dev, float* lse_c_dev,
+                    void* ws_dev, long long ws_bytes, void* stream);
+int mk_dual_softmax_backward(const float* dsc0_dev, const float* dsc1_dev, const float* scr0_dev, const float* scr1_dev,
+                             const float* dustbin_dev, float temperature, int B, int N, const float* lse_r_dev,
+                             const float* lse_c_dev, const float* grad_scores_dev, long long gs_pitch, const float* grad_kp_dev,
+                             long long gk_pitch, const float* grad_final_dev, long long gf_pitch, float* ddsc0_dev,
+                             float* ddsc1_dev, float* dscr0_dev, float* dscr1_dev, float* ddustbin_dev, void* ws_dev,
+                             long long ws_bytes, void* stream);
+
 /* (Re)seed the solver's device-side generator on `stream` (used in front of a CUDA-graph replay of mk_forward
  * captured with seed = 0). */
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream);

@@ -105,6 +105,15 @@ EXPORTS = {
     "mk_loss_gradient": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
     "mk_loss_gradient_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int]),
+    "mk_dual_softmax_ws_bytes": (C.c_longlong, [C.c_int, C.c_int]),
+    "mk_dual_softmax_backward_ws_bytes": (C.c_longlong, [C.c_int, C.c_int]),
+    "mk_dual_softmax": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int,
+                                  C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_dual_softmax_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int,
+                                           C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p,
+                                           C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
     "mk_pose_to_submission": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "mk_launch_count": (C.c_longlong, [C.c_void_p]),
     "mk_pdl_enabled": (C.c_int, []),
