@@ -317,6 +317,10 @@ int mk_op_matcher_reduce(const float* part_row, const float* part_col, const flo
 int mk_op_sample(const float* final_scores, int B, int N, long long pitch, int IM, int n_sample, unsigned long long seed, void* ws,
                  long long ws_bytes, int* idx_out, int* status, void* stream);
 long long mk_op_sample_workspace_bytes(int B, int IM);
+/* The solver's fp64 Kabsch rotation on n matrices, one per thread: H, R device [n, 9] row-major.  R is the rotation
+   maximising tr(R H) (det R = +1); H == 0 gives the identity, a NaN or +-inf anywhere in H gives nine NaNs.
+   MK_ERR_INVALID for n < 0 or a null pointer. */
+int mk_op_kabsch(const double* H, double* R, int n, void* stream);
 
 #ifdef __cplusplus
 }

@@ -133,6 +133,7 @@ EXPORTS = {
     "mk_op_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_ulonglong, C.c_void_p, C.c_longlong,
                                C.c_void_p, C.c_void_p, C.c_void_p]),
     "mk_op_sample_workspace_bytes": (C.c_longlong, [C.c_int, C.c_int]),
+    "mk_op_kabsch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
 }
 
 _lib = None

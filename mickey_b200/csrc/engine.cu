@@ -766,5 +766,6 @@ int mk_op_sample(const float* fs, int B, int N, long long pitch, int IM, int n_s
   MK_TRY(seed_set(sd, seed, (cudaStream_t)stream));
   return sample_outer(fs, B, N, pitch, IM, n_sample, sd, ws, idx_out, status, (cudaStream_t)stream);
 }
+int mk_op_kabsch(const double* H, double* R, int n, void* stream) { return kabsch_batch(H, R, n, (cudaStream_t)stream); }
 
 }  // extern "C"

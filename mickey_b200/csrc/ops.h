@@ -52,6 +52,8 @@ int ransac_solve(const float* final_scores, long long pitch, const float* kps0, 
                  const float* K0, const float* K1, int B, int N, const RansacParams& rp, const int* outer_idx,
                  const int* inner_idx, float* hyp_scores, float* hyp_Rt, int* counters, float* pose,
                  int* best_set, float* inl_mask, int* best_hyp, cudaStream_t st);
+// H [n][9], R [n][9] fp64 row-major, device: R = kabsch_rotation(H) per matrix (ransac_dev.cuh)
+int kabsch_batch(const double* H, double* R, int n, cudaStream_t st);
 constexpr int SOLVER_COUNTER_BASE = 4;      // counters: [0] status bits, [1] pairs finished, [4 + b] blocks of pair b finished
 
 // loss.cu: MetricPoseLoss's draws, refinement search and REINFORCE gradient (include/mickey_b200.h mk_loss_search)

@@ -895,4 +895,20 @@ int ransac_solve(const float* final_scores, long long pitch, const float* kps0, 
   return MK_OK;
 }
 
+// the Kabsch rotation alone, one 3x3 H per thread: the solver's and the loss's kabsch_rotation, exposed for tests
+__global__ void kabsch_kernel(const double* __restrict__ H, double* __restrict__ R, int n) {
+  pdl_wait();
+  pdl_trigger();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  kabsch_rotation(H + (long long)i * 9, R + (long long)i * 9);
+}
+
+int kabsch_batch(const double* H, double* R, int n, cudaStream_t st) {
+  if (n < 0 || !H || !R) { set_last_error("kabsch: n must be >= 0 and H, R non-null"); return MK_ERR_INVALID; }
+  if (n == 0) return MK_OK;
+  MK_CUDA_CHECK(launch_k(kabsch_kernel, dim3((unsigned)ceil_div(n, 128)), dim3(128), 0, st, H, R, n));
+  return MK_OK;
+}
+
 }  // namespace mk

@@ -83,12 +83,37 @@ __device__ __forceinline__ void gather_set(const int* __restrict__ idx, const fl
 // factors are proper rotations, so R = V U^T already has det +1 and equals the reference's sign-fixed product for
 // every rank >= 2 matrix (3-point hypotheses are always rank <= 2: the third singular direction is a cross product,
 // not a division by ~0).
-__device__ inline void kabsch_rotation(const double* Hin, double* R) {
+// H is first scaled by the power of two that puts max|H_ij| in [1, 2): R does not depend on the scale, every step of
+// the sweep is homogeneous in it and a power-of-two scale is exact, so R is bit-identical to the unscaled sweep wherever
+// both stay in the normal range, and the absolute guards below (1e-300) mean the same thing at every scale.  A NaN or
+// +-inf anywhere in H gives R = NaN in all nine entries; H == 0 gives the identity.
+// __host__ __device__ so that host tests can build the same function (tests/test_kabsch_host.py).
+__host__ __device__ inline void kabsch_rotation(const double* Hin, double* R) {
   double A[3][3], V[3][3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}};
+  double hmax = 0.0;
+  bool finite = true;
+#pragma unroll
+  for (int i = 0; i < 9; ++i) {
+    const double a = fabs(Hin[i]);
+    finite = finite && a <= 1.7976931348623157e308;            // false for NaN and +-inf
+    hmax = fmax(hmax, a);
+  }
+  if (!finite) {
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R[i] = nan("");
+    return;
+  }
+  if (hmax == 0.0) {     // H == 0: identity
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R[i] = (i % 4 == 0) ? 1.0 : 0.0;
+    return;
+  }
+  int ex;
+  frexp(hmax, &ex);                                             // hmax = m 2^ex, m in [0.5, 1)
 #pragma unroll
   for (int i = 0; i < 3; ++i)
 #pragma unroll
-    for (int j = 0; j < 3; ++j) A[i][j] = Hin[i * 3 + j];
+    for (int j = 0; j < 3; ++j) A[i][j] = ldexp(Hin[i * 3 + j], 1 - ex);
   for (int sweep = 0; sweep < 12; ++sweep) {
     double off = 0.0;
 #pragma unroll
@@ -123,13 +148,8 @@ __device__ inline void kabsch_rotation(const double* Hin, double* R) {
   int i2 = (i1 + 1) % 3, i3 = (i1 + 2) % 3;
   if (sg[i3] > sg[i2]) { const int tmp = i2; i2 = i3; i3 = tmp; }
   double u1[3], u2[3], v1[3], v2[3];
+  // s1 > 0.5: the scaled H has an entry >= 1, and the rotations keep the Frobenius norm, so max_j sg[j]^2 >= 1/3
   const double s1 = sg[i1], s2 = sg[i2];
-  if (!(s1 > 0.0)) {     // H == 0 (or NaN): identity (NaN inputs propagate through t and are flagged by the caller)
-#pragma unroll
-    for (int i = 0; i < 9; ++i) R[i] = (i % 4 == 0) ? 1.0 : 0.0;
-    if (s1 != s1) R[0] = s1;
-    return;
-  }
 #pragma unroll
   for (int i = 0; i < 3; ++i) { u1[i] = A[i][i1] / s1; v1[i] = V[i][i1]; v2[i] = V[i][i2]; }
   if (s2 > 1e-14 * s1) {
