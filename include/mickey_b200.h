@@ -88,6 +88,21 @@ int mk_extract_images(mk_handle* h, const float* images_dev, int n_img, int img_
 int mk_extract_images_u8(mk_handle* h, const unsigned char* images_u8_dev, int n_img, int img_h, int img_w, float* kps_dev,
                          float* depth_dev, float* scr_dev, float* dsc_dev, void* ws_dev, long long ws_bytes, void* stream);
 
+/* ---- training: the frozen DINOv2 backbone alone (mickey_b200/dinov2.py wraps it as a drop-in module).  Replaces
+ * DinoVisionTransformer.forward_features (dinov2.py:221-236) followed by the extractor's
+ * x_norm_patchtokens.permute(0, 2, 1).reshape(B, C, h, w).float() (mickey_extractor.py:49-51), so that the heads can
+ * run in torch in train mode.
+ * images_dev fp32 [n_img, 3, H, W] (H, W multiples of 14, at least 98, equal to the finalized geometry); the patch
+ * gather, the patch embedding and every block run exactly as in mk_extract, then the final LayerNorm writes out_dev fp32
+ * [n_img, D, N] channel-major (cls token dropped).  out rounded to fp16 is bit for bit the feature image mk_extract
+ * gives the heads.  Only the backbone's tensors need to be registered.  Workspace: mk_backbone_ws_bytes(n_img, H, W)
+ * bytes; it holds the six backbone buffers ("P", "X", "XN", "QKV", "ATT", "H1") at the offsets mk_workspace_offset names
+ * for n_img images.  Bad arguments (a NULL pointer, n_img < 1, a bad geometry, an unfinalized handle, a small workspace)
+ * return MK_ERR_INVALID and launch nothing.  mk_backbone_ws_bytes returns -1 for a bad geometry or count. */
+long long mk_backbone_ws_bytes(mk_handle* h, int n_img, int img_h, int img_w);
+int mk_backbone_features(mk_handle* h, const float* images_dev, int n_img, int img_h, int img_w, float* out_dev,
+                         void* ws_dev, long long ws_bytes, void* stream);
+
 /* ---- stage 2: dual-softmax matcher
  * replaces featureMatcher/dualSoftmax.forward (feature_matcher.py:48-83), kp_matrix_scores
  * (compute_correspondences.py:46-50) and `final_scores = scores * kp_scores` (compute_pose.py:23).

@@ -76,20 +76,34 @@ struct Workspace {
   size_t bytes;
 };
 
-Workspace carve(void* base, const mk_config& c, const Geo& g) {
-  Workspace w;
-  Carver cv(base);
-  const int n_pairs = g.n_pairs;
-  const size_t D = c.embed_dim, M = g.M, R = g.R;
-  // the matcher's operands: written by the extraction (n_img images) or by the bank gather (2 * n_pairs role rows)
-  const size_t n_op = (size_t)std::max(g.n_img, 2 * g.n_pairs);
-  const int* bd = c.block_dims;
+// The backbone's six buffers open every workspace, so a backbone-only call (mk_backbone_features) carves just them and
+// they sit at the same offsets as in the full workspace of the same image count.
+void carve_backbone(Carver& cv, const mk_config& c, const Geo& g, Workspace& w) {
+  const size_t D = c.embed_dim, M = g.M;
   w.P = cv.take<__half>((size_t)g.Mp * KPAD);
   w.X = cv.take<float>(M * D);
   w.XN = cv.take<__half>(M * D);
   w.QKV = cv.take<__half>(M * 3 * D);
   w.ATT = cv.take<__half>(M * D);
   w.H1 = cv.take<__half>(M * 4 * D);
+}
+
+size_t backbone_ws_bytes(const mk_config& c, const Geo& g) {
+  Carver cv(nullptr);
+  Workspace w;
+  carve_backbone(cv, c, g, w);
+  return (cv.off + 255) & ~(size_t)255;
+}
+
+Workspace carve(void* base, const mk_config& c, const Geo& g) {
+  Workspace w;
+  Carver cv(base);
+  const int n_pairs = g.n_pairs;
+  const size_t D = c.embed_dim, R = g.R;
+  // the matcher's operands: written by the extraction (n_img images) or by the bank gather (2 * n_pairs role rows)
+  const size_t n_op = (size_t)std::max(g.n_img, 2 * g.n_pairs);
+  const int* bd = c.block_dims;
+  carve_backbone(cv, c, g, w);
   w.F = cv.take<__half>(R * D);
   w.T1 = cv.take<__half>(R * G * bd[0]); w.S1 = cv.take<__half>(R * G * bd[0]); w.O1 = cv.take<__half>(R * G * bd[0]);
   w.T2 = cv.take<__half>(R * G * bd[1]); w.S2 = cv.take<__half>(R * G * bd[1]); w.O2 = cv.take<__half>(R * G * bd[1]);
@@ -180,9 +194,9 @@ int gemm(mk_handle* h, const char* tag, int epi, const void* a, long long a_rows
 #define MK_KERNEL(tag, call) do { ProfScope ps_(h, tag, st); h->launches++; MK_TRY(call); } while (0)
 
 // ---- stage 1 ----------------------------------------------------------------------------------------------
+// The DINOv2 backbone up to (not including) the final norm: the residual stream of every token ends in w.X.
 // img_fmt 0: fp32 NCHW in [0,1] (the reference's tensors); 1: uint8 NHWC RGB as cv2 delivers it (mk_*_u8, SURVEY.md §8 f1)
-int run_extract(mk_handle* h, const void* images, int img_fmt, const Geo& g, float* kps, float* depth, float* scr,
-                float* dsc, Workspace& w, cudaStream_t st) {
+int run_backbone(mk_handle* h, const void* images, int img_fmt, const Geo& g, Workspace& w, cudaStream_t st) {
   const mk_config& c = h->cfg;
   const int H = g.H, W = g.W;
   const int D = c.embed_dim;
@@ -231,6 +245,15 @@ int run_extract(mk_handle* h, const void* images, int img_fmt, const Geo& g, flo
       }
       MK_TRY(gemm(h, "vit.fc2", fuse_next ? EPI_RESID_LN : EPI_RESID_F, w.H1, g.M, 4 * D, wfc2, D, 4 * D, p, st)); }
   }
+  return MK_OK;
+}
+
+int run_extract(mk_handle* h, const void* images, int img_fmt, const Geo& g, float* kps, float* depth, float* scr,
+                float* dsc, Workspace& w, cudaStream_t st) {
+  const mk_config& c = h->cfg;
+  const int D = c.embed_dim;
+  Lookup L{h};
+  MK_TRY(run_backbone(h, images, img_fmt, g, w, st));
   // -- final norm, drop cls, scatter into the zero-padded NHWC feature image (dinov2.py:230-233, mickey_extractor.py:49-51)
   MK_CUDA_CHECK(cudaMemsetAsync(w.F, 0, (size_t)g.R * D * sizeof(__half), st));
   MK_KERNEL("vit.layernorm", layernorm(w.X, L.f("norm.w", D), L.f("norm.b", D), w.F, (int)g.M, D, 1e-6f, 1, g.gh, g.gw, st));
@@ -543,6 +566,46 @@ int mk_extract_images(mk_handle* h, const float* images, int n_img, int H, int W
 int mk_extract_images_u8(mk_handle* h, const unsigned char* images, int n_img, int H, int W, float* kps, float* depth, float* scr,
                          float* dsc, void* ws, long long ws_bytes, void* stream) {
   return extract_images_any(h, images, 1, n_img, H, W, kps, depth, scr, dsc, ws, ws_bytes, stream);
+}
+
+long long mk_backbone_ws_bytes(mk_handle* h, int n_img, int H, int W) {
+  if (!h || n_img < 1 || H < 98 || W < 98 || H % 14 || W % 14) return -1;
+  return (long long)backbone_ws_bytes(h->cfg, make_geo(n_img, 0, H, W));
+}
+
+int mk_backbone_features(mk_handle* h, const float* images, int n_img, int H, int W, float* out, void* ws, long long ws_bytes,
+                         void* stream) {
+  // every argument is checked before the handle is read and before anything is launched
+  if (!h || !images || !out || !ws) { set_last_error("mk_backbone_features: null argument"); return MK_ERR_INVALID; }
+  if (n_img < 1) { set_last_error("mk_backbone_features: n_img %d must be positive", n_img); return MK_ERR_INVALID; }
+  if (H < 98 || W < 98 || H % 14 || W % 14) {
+    set_last_error("mk_backbone_features: image %dx%d must be multiples of 14 and at least 98", H, W);
+    return MK_ERR_INVALID;
+  }
+  if (!h->finalized) { set_last_error("mk_backbone_features: handle not finalized"); return MK_ERR_INVALID; }
+  if (H != h->geo_h || W != h->geo_w) {
+    set_last_error("mk_backbone_features: geometry %dx%d does not match the finalized geometry %dx%d", H, W, h->geo_h, h->geo_w);
+    return MK_ERR_INVALID;
+  }
+  const Geo g = make_geo(n_img, 0, H, W);
+  const size_t need = backbone_ws_bytes(h->cfg, g);
+  if ((long long)need > ws_bytes) {
+    set_last_error("mk_backbone_features: workspace too small: need %zu bytes, got %lld", need, ws_bytes);
+    return MK_ERR_INVALID;
+  }
+  MK_CUDA_CHECK(cudaSetDevice(h->device));
+  const int D = h->cfg.embed_dim;
+  Lookup L{h};
+  const float *nw = L.f("norm.w", D), *nb = L.f("norm.b", D);
+  if (!L.ok) return MK_ERR_MISSING_TENSOR;
+  Workspace w;
+  Carver cv(ws);
+  carve_backbone(cv, h->cfg, g, w);
+  cudaStream_t st = (cudaStream_t)stream;
+  MK_TRY(run_backbone(h, images, 0, g, w, st));
+  // -- final norm, drop cls, channel-major fp32 (dinov2.py:230-233, mickey_extractor.py:49-51)
+  MK_KERNEL("vit.layernorm_cm", layernorm_channel_major(w.X, nw, nb, out, n_img, g.N, D, 1e-6f, st));
+  return MK_OK;
 }
 
 int mk_match(mk_handle* h, int n_pairs, float* scores, float* kp_scores, float* final_scores, long long nn_pitch, void* ws,

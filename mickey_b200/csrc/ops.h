@@ -7,6 +7,9 @@ namespace mk {
 // vit_ops.cu
 int patch_gather(const float* img, void* P, int n_img, int H, int W, int kpad, float* X, const float* cls_pos, int D, cudaStream_t s);
 int layernorm(const float* x, const float* w, const float* b, void* out, int rows, int D, float eps, int mode, int gh, int gw, cudaStream_t s);
+// the final norm as fp32 channel-major [n_img, D, N] from the residual [n_img * (N + 1), D] (cls row dropped)
+int layernorm_channel_major(const float* x, const float* w, const float* b, float* out, int n_img, int N, int D, float eps,
+                            cudaStream_t s);
 int attention(const void* qkv, void* out, int n_img, int T, int D, int heads, cudaStream_t s);      // mma.sync version (v1, kept as a cross-check)
 int attention_tc(const void* qkv, void* out, int n_img, int T, int D, int heads, cudaStream_t s);   // wgmma / TMA version
 int attention_dispatch(const void* qkv, void* out, int n_img, int T, int D, int heads, int impl, cudaStream_t s);

@@ -48,7 +48,38 @@ int patch_gather(const float* img, void* P, int n_img, int H, int W, int kpad, f
 // mode 1: final norm (dinov2.py:230-233): drop the cls token and scatter patch tokens into the
 //         zero-padded NHWC feature image that feeds the head convolutions:
 //         out[(img*(gh+2) + y+1)*(gw+2) + x+1][:] = LN(x[img*T + 1 + y*gw + x])
+// mode 2 (layernorm_cm_kernel): the same final norm written as the heads' fp32 input, channel-major [n_img, D, N]
+//         (mickey_extractor.py:49-51: x_norm_patchtokens.permute(0, 2, 1).reshape(B, C, h, w).float()).
+// All modes share ln_row_stats / ln_affine: one summation order, one expression, so mode 2's value rounded to fp16
+// is mode 1's F interior bit for bit.
 // ------------------------------------------------------------------------------------------------------
+// One warp reads one row (lane holds float4s i*32 + lane) and reduces its mean and 1 / std.
+template <int VEC>
+__device__ __forceinline__ void ln_row_stats(const float* __restrict__ xrow, int lane, int D, float eps, float4 (&v)[VEC],
+                                             float& mean, float& rstd) {
+  const float4* xr = reinterpret_cast<const float4*>(xrow);
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) {
+    v[i] = xr[i * 32 + lane];
+    sum += v[i].x + v[i].y + v[i].z + v[i].w;
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  mean = sum / D;
+  float sq = 0.f;
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) {
+    const float a = v[i].x - mean, c = v[i].y - mean, d = v[i].z - mean, e = v[i].w - mean;
+    sq += a * a + c * c + d * d + e * e;
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+  rstd = rsqrtf(sq / D + eps);
+}
+
+__device__ __forceinline__ float ln_affine(float v, float mean, float rstd, float w, float b) { return (v - mean) * rstd * w + b; }
+
 template <int VEC>   // D = 128 * VEC
 __global__ void layernorm_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
                                  __half* __restrict__ out, int rows, int D, float eps, int mode, int gh, int gw) {
@@ -65,39 +96,83 @@ __global__ void layernorm_kernel(const float* __restrict__ x, const float* __res
     const int y = (t - 1) / gw, xx = (t - 1) % gw;
     orow = ((long long)im * (gh + 2) + y + 1) * (gw + 2) + xx + 1;
   }
-  const float4* xr = reinterpret_cast<const float4*>(x + (size_t)row * D);
   float4 v[VEC];
-  float sum = 0.f;
-#pragma unroll
-  for (int i = 0; i < VEC; ++i) {
-    v[i] = xr[i * 32 + lane];
-    sum += v[i].x + v[i].y + v[i].z + v[i].w;
-  }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float mean = sum / D;
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < VEC; ++i) {
-    const float a = v[i].x - mean, c = v[i].y - mean, d = v[i].z - mean, e = v[i].w - mean;
-    sq += a * a + c * c + d * d + e * e;
-  }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  const float rstd = rsqrtf(sq / D + eps);
+  float mean, rstd;
+  ln_row_stats<VEC>(x + (size_t)row * D, lane, D, eps, v, mean, rstd);
   __half* orow_p = out + (size_t)orow * D;
 #pragma unroll
   for (int i = 0; i < VEC; ++i) {
     const int c0 = (i * 32 + lane) * 4;
     const float4 ww = *reinterpret_cast<const float4*>(w + c0);
     const float4 bb = *reinterpret_cast<const float4*>(b + c0);
-    __half2 h0 = __floats2half2_rn((v[i].x - mean) * rstd * ww.x + bb.x, (v[i].y - mean) * rstd * ww.y + bb.y);
-    __half2 h1 = __floats2half2_rn((v[i].z - mean) * rstd * ww.z + bb.z, (v[i].w - mean) * rstd * ww.w + bb.w);
+    __half2 h0 = __floats2half2_rn(ln_affine(v[i].x, mean, rstd, ww.x, bb.x), ln_affine(v[i].y, mean, rstd, ww.y, bb.y));
+    __half2 h1 = __floats2half2_rn(ln_affine(v[i].z, mean, rstd, ww.z, bb.z), ln_affine(v[i].w, mean, rstd, ww.w, bb.w));
     uint2 u;
     u.x = *reinterpret_cast<uint32_t*>(&h0);
     u.y = *reinterpret_cast<uint32_t*>(&h1);
     *reinterpret_cast<uint2*>(orow_p + c0) = u;
   }
+}
+
+// Final norm into the channel-major [n_img, D, N] fp32 feature map.  A CTA takes LNCM_TOK consecutive patch tokens of
+// one image (grid: ceil(N / LNCM_TOK) x n_img); each of its 16 warps normalises two of them with the row reads of
+// layernorm_kernel (512-byte coalesced float4 loads).  The normalised tile leaves 128 channels at a time through a
+// [128][LNCM_TOK + 1] shared-memory transpose: one warp stores 32 consecutive tokens of one channel (128 bytes).
+constexpr int LNCM_TOK = 32, LNCM_WARPS = 16, LNCM_ROWS = LNCM_TOK / LNCM_WARPS;
+
+template <int VEC>   // D = 128 * VEC
+__global__ void __launch_bounds__(LNCM_WARPS * 32)
+layernorm_cm_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
+                    float* __restrict__ out, int N, int D, float eps) {
+  __shared__ float tile[128][LNCM_TOK + 1];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int im = blockIdx.y, t0 = blockIdx.x * LNCM_TOK;
+  pdl_wait();
+  pdl_trigger();
+  float4 v[LNCM_ROWS][VEC];
+  float mean[LNCM_ROWS], rstd[LNCM_ROWS];
+#pragma unroll
+  for (int r = 0; r < LNCM_ROWS; ++r) {
+    const int t = min(t0 + warp * LNCM_ROWS + r, N - 1);        // rows past N repeat the last token; never stored
+    ln_row_stats<VEC>(x + ((size_t)im * (N + 1) + 1 + t) * D, lane, D, eps, v[r], mean[r], rstd[r]);
+  }
+  float* obase = out + (size_t)im * D * N;
+  const int t_out = t0 + lane;
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) {
+    const int c0 = (i * 32 + lane) * 4;
+    const float4 ww = *reinterpret_cast<const float4*>(w + c0);
+    const float4 bb = *reinterpret_cast<const float4*>(b + c0);
+#pragma unroll
+    for (int r = 0; r < LNCM_ROWS; ++r) {
+      const int tt = warp * LNCM_ROWS + r;
+      tile[lane * 4 + 0][tt] = ln_affine(v[r][i].x, mean[r], rstd[r], ww.x, bb.x);
+      tile[lane * 4 + 1][tt] = ln_affine(v[r][i].y, mean[r], rstd[r], ww.y, bb.y);
+      tile[lane * 4 + 2][tt] = ln_affine(v[r][i].z, mean[r], rstd[r], ww.z, bb.z);
+      tile[lane * 4 + 3][tt] = ln_affine(v[r][i].w, mean[r], rstd[r], ww.w, bb.w);
+    }
+    __syncthreads();
+    if (t_out < N) {
+#pragma unroll
+      for (int k = 0; k < 128 / LNCM_WARPS; ++k) {
+        const int c = k * LNCM_WARPS + warp;
+        obase[(size_t)(i * 128 + c) * N + t_out] = tile[c][lane];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+int layernorm_channel_major(const float* x, const float* w, const float* b, float* out, int n_img, int N, int D, float eps,
+                            cudaStream_t s) {
+  dim3 grid(ceil_div(N, LNCM_TOK), n_img), block(LNCM_WARPS * 32);
+  switch (D) {
+    case 384:  MK_CUDA_CHECK(launch_k(layernorm_cm_kernel<3>, grid, block, 0, s, x, w, b, out, N, D, eps)); break;
+    case 768:  MK_CUDA_CHECK(launch_k(layernorm_cm_kernel<6>, grid, block, 0, s, x, w, b, out, N, D, eps)); break;
+    case 1024: MK_CUDA_CHECK(launch_k(layernorm_cm_kernel<8>, grid, block, 0, s, x, w, b, out, N, D, eps)); break;
+    default: set_last_error("layernorm: unsupported width %d", D); return MK_ERR_UNSUPPORTED;
+  }
+  return MK_OK;
 }
 
 int layernorm(const float* x, const float* w, const float* b, void* out, int rows, int D, float eps, int mode, int gh,

@@ -86,23 +86,26 @@ def _fold_conv3x3(w: torch.Tensor, bn: Optional[Dict[str, torch.Tensor]]):
     return wp, shift
 
 
-def pack_weights(sd: Dict[str, torch.Tensor], cfg, device) -> Dict[str, torch.Tensor]:
-    """state dict with reference names (fp32 or fp16) -> {packed name: device tensor}."""
-    variant = backbone_variant(cfg)
+def _h16(t):
+    return t.to(torch.float16).contiguous()
+
+
+def _f32(t):
+    return t.to(torch.float32).contiguous()
+
+
+def pack_backbone(sd: Dict[str, torch.Tensor], variant: str, device, prefix: str = BACKBONE) -> Dict[str, torch.Tensor]:
+    """The DINOv2 backbone's tensors of a state dict (fp32 or fp16; names `prefix` + the reference's module names) ->
+    {packed name: device tensor}: the patch embedding, every block and the final norm.  The size-dependent tables
+    (position embedding, cls token, patch bias) are built per image geometry by whoever finalizes the handle."""
     D, depth, _ = VARIANTS[variant]
-    use_bn = bool(cfg["MICKEY"]["KP_HEADS"]["BN"])
     out: Dict[str, torch.Tensor] = {}
 
     def g(name):
         return sd[name].detach().to(device)
 
-    def h16(t):
-        return t.to(torch.float16).contiguous()
-
-    def f32(t):
-        return t.to(torch.float32).contiguous()
-
-    b = BACKBONE
+    h16, f32 = _h16, _f32
+    b = prefix
     pw = g(b + "patch_embed.proj.weight").float().reshape(D, 3 * PATCH * PATCH)
     out["patch.w"] = h16(F.pad(pw, (0, KPAD - pw.shape[1])))
     for i in range(depth):
@@ -115,6 +118,18 @@ def pack_weights(sd: Dict[str, torch.Tensor], cfg, device) -> Dict[str, torch.Te
         out[q + "fc2.w"], out[q + "fc2.b"] = h16(g(p + "mlp.fc2.weight")), f32(g(p + "mlp.fc2.bias"))
         out[q + "ls1"], out[q + "ls2"] = f32(g(p + "ls1.gamma")), f32(g(p + "ls2.gamma"))
     out["norm.w"], out["norm.b"] = f32(g(b + "norm.weight")), f32(g(b + "norm.bias"))
+    return out
+
+
+def pack_weights(sd: Dict[str, torch.Tensor], cfg, device) -> Dict[str, torch.Tensor]:
+    """state dict with reference names (fp32 or fp16) -> {packed name: device tensor}."""
+    use_bn = bool(cfg["MICKEY"]["KP_HEADS"]["BN"])
+    out = pack_backbone(sd, backbone_variant(cfg), device)
+
+    def g(name):
+        return sd[name].detach().to(device)
+
+    h16, f32 = _h16, _f32
 
     def bn_of(prefix):
         if not use_bn:
