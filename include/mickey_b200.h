@@ -271,6 +271,42 @@ int mk_dual_softmax_backward(const float* dsc0_dev, const float* dsc1_dev, const
                              float* ddsc1_dev, float* dscr0_dev, float* dscr1_dev, float* ddustbin_dev, void* ws_dev,
                              long long ws_bytes, void* stream);
 
+/* ---- training: the heads' linear-attention transformer, Transformer_self_att (att_layers/transformer.py:75-103), forward
+ * and backward (mickey_b200/head_transformer.py wraps both as a torch.autograd.Function).  No handle: the parameters change
+ * at every optimizer step, so every call takes the caller's parameter pointers, one table per layer.
+ *
+ * Every parameter is an fp32 device pointer, contiguous and 16-byte aligned, in the reference's layout: q_proj, k_proj,
+ * v_proj and merge [128, 128], mlp0 [256, 256] (mlp.0), mlp2 [128, 256] (mlp.2), norm1_w / norm1_b / norm2_w / norm2_b
+ * [128].  In mk_htr_layer_grads the same names are the gradients to write (overwritten, not accumulated); NULL skips one.
+ *
+ * mk_head_transformer: x_dev fp32 [B, 128, h, w] contiguous, pe_dev the positional encoding [128, 256, 256] (posEnc.pe,
+ * added as pe[:, :h, :w]) or NULL, out_dev fp32 [B, 128, h, w].  save = 1 keeps every layer's activations in the
+ * workspace for mk_head_transformer_backward, which reads them from that workspace (saved_dev); save = 0 runs the forward
+ * only, in a smaller workspace.  The output is the same bits either way.
+ * mk_head_transformer_backward: grad_out_dev fp32 [B, 128, h, w] contiguous; grad_x_dev fp32 [B, 128, h, w] or NULL.
+ * grads_host is an array of num_layers tables.  Only what a requested gradient needs is computed.
+ *
+ * All arithmetic is fp32 (FMA on the CUDA cores).  Both calls are deterministic, use no atomics, and an image's output and
+ * input gradient are the same bits alone and inside a batch (weight gradients sum over the batch).  Workspaces:
+ * mk_head_transformer_ws_bytes / mk_head_transformer_backward_ws_bytes bytes (-1 for a bad geometry: B, h, w >= 1,
+ * 1 <= num_layers <= 1024, B <= 65535, B h w <= 4,194,240 = 65535 * 64).  Bad arguments return MK_ERR_INVALID and
+ * launch nothing. */
+typedef struct mk_htr_layer {
+  const float* q_proj; const float* k_proj; const float* v_proj; const float* merge; const float* mlp0; const float* mlp2;
+  const float* norm1_w; const float* norm1_b; const float* norm2_w; const float* norm2_b;
+} mk_htr_layer;
+typedef struct mk_htr_layer_grads {
+  float* q_proj; float* k_proj; float* v_proj; float* merge; float* mlp0; float* mlp2;
+  float* norm1_w; float* norm1_b; float* norm2_w; float* norm2_b;
+} mk_htr_layer_grads;
+long long mk_head_transformer_ws_bytes(int B, int h, int w, int num_layers, int save);
+long long mk_head_transformer_backward_ws_bytes(int B, int h, int w, int num_layers);
+int mk_head_transformer(const float* x_dev, const float* pe_dev, int B, int h, int w, const mk_htr_layer* layers_host,
+                        int num_layers, float* out_dev, int save, void* ws_dev, long long ws_bytes, void* stream);
+int mk_head_transformer_backward(const void* saved_dev, const float* grad_out_dev, int B, int h, int w,
+                                 const mk_htr_layer* layers_host, int num_layers, float* grad_x_dev,
+                                 mk_htr_layer_grads* grads_host, void* ws_dev, long long ws_bytes, void* stream);
+
 /* (Re)seed the solver's device-side generator on `stream` (used in front of a CUDA-graph replay of mk_forward
  * captured with seed = 0). */
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream);

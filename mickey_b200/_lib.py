@@ -55,6 +55,14 @@ class MkGemmArgs(C.Structure):
     ]
 
 
+class MkHtrLayer(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("q_proj", "k_proj", "v_proj", "merge", "mlp0", "mlp2",
+                                          "norm1_w", "norm1_b", "norm2_w", "norm2_b")]
+
+
+MkHtrLayerGrads = MkHtrLayer     # the same ten pointers, written instead of read
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "mk_create": (C.c_int, [C.c_int, C.POINTER(MkConfig), C.POINTER(C.c_void_p)]),
@@ -117,6 +125,13 @@ EXPORTS = {
                                            C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p,
                                            C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_head_transformer_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_head_transformer_backward_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_head_transformer": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(MkHtrLayer), C.c_int,
+                                      C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_head_transformer_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(MkHtrLayer),
+                                               C.c_int, C.c_void_p, C.POINTER(MkHtrLayerGrads), C.c_void_p, C.c_longlong,
+                                               C.c_void_p]),
     "mk_pose_to_submission": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "mk_launch_count": (C.c_longlong, [C.c_void_p]),
     "mk_pdl_enabled": (C.c_int, []),
