@@ -307,6 +307,61 @@ int mk_head_transformer_backward(const void* saved_dev, const float* grad_out_de
                                  const mk_htr_layer* layers_host, int num_layers, float* grad_x_dev,
                                  mk_htr_layer_grads* grads_host, void* ws_dev, long long ws_bytes, void* stream);
 
+/* ---- training: the heads' residual block, BasicBlock (extractor_utils.py:12-35), forward and backward with TF32 wgmma
+ * convolutions and batch norm (mickey_b200/resblock.py wraps both as a torch.autograd.Function).  No handle: every call
+ * takes the caller's parameter pointers, because the parameters change at every optimizer step.
+ *
+ * Parameters are fp32 device pointers, contiguous, in the torch layout: w1 [cout, cin, 3, 3], w2 [cout, cout, 3, 3], wsc
+ * [cout, cin, 1, 1] (exactly when cin != cout; NULL for the identity shortcut), the BN weights, biases and running
+ * statistics [cout].  momentum1 / momentum2 are the exponential-average factors of this call (the module's momentum, or
+ * 1 / num_batches_tracked for the cumulative average); running_var receives the unbiased batch variance.
+ *
+ * mk_resblock_forward: x_dev fp32 [B, cin, h, w] with element strides x_strides_host[4] (any layout); out_dev fp32
+ * [B, cout, h, w] contiguous.  flags: MK_RB_TRAIN (batch statistics, running statistics updated; otherwise the running
+ * statistics normalise and nothing is updated), MK_RB_RELU (the final ReLU), MK_RB_BN (batch norm present; otherwise
+ * both BN layers are identities), MK_RB_SAVE (also write the channel-major operand copies the backward needs).  saved_dev
+ * (mk_resblock_saved_bytes) receives what mk_resblock_backward reads; ws_dev (mk_resblock_ws_bytes) is scratch that can
+ * be freed when the forward has run.
+ * mk_resblock_backward: grad_out_dev fp32 [B, cout, h, w] with element strides g_strides_host[4]; out_dev the forward's
+ * output (its ReLU mask; may be NULL without MK_RB_RELU); flags as in the forward.  want is a mask of MK_RB_GRAD_* bits; a
+ * requested gradient's pointer in grads_host must be set, and each is overwritten, not accumulated.  Contractions whose
+ * results nobody wants are skipped: without MK_RB_GRAD_X there is no data gradient through conv1 or the shortcut.
+ *
+ * Channel counts are multiples of 32 in [32, 4096], B, h, w >= 1 and B (h+2)(w+2) <= 2^24; training-mode batch norm
+ * needs B h w >= 2.  Workspace sizes: -1 for a bad geometry.  Bad arguments return MK_ERR_INVALID and launch nothing.
+ * Deterministic: no atomics, bit-identical run to run. */
+#define MK_RB_TRAIN 1
+#define MK_RB_RELU 2
+#define MK_RB_SAVE 4
+#define MK_RB_BN 8
+#define MK_RB_GRAD_X 1
+#define MK_RB_GRAD_W1 2
+#define MK_RB_GRAD_W2 4
+#define MK_RB_GRAD_WSC 8
+#define MK_RB_GRAD_BN1_W 16
+#define MK_RB_GRAD_BN1_B 32
+#define MK_RB_GRAD_BN2_W 64
+#define MK_RB_GRAD_BN2_B 128
+typedef struct mk_resblock_params {
+  const float* w1; const float* w2; const float* wsc;
+  const float* bn1_w; const float* bn1_b; float* bn1_mean; float* bn1_var;
+  const float* bn2_w; const float* bn2_b; float* bn2_mean; float* bn2_var;
+  float eps1, eps2, momentum1, momentum2;
+} mk_resblock_params;
+typedef struct mk_resblock_grads {
+  float* dx; float* w1; float* w2; float* wsc; float* bn1_w; float* bn1_b; float* bn2_w; float* bn2_b;
+} mk_resblock_grads;
+long long mk_resblock_ws_bytes(int B, int h, int w, int cin, int cout);
+long long mk_resblock_saved_bytes(int B, int h, int w, int cin, int cout);
+long long mk_resblock_backward_ws_bytes(int B, int h, int w, int cin, int cout);
+int mk_resblock_forward(const float* x_dev, const long long* x_strides_host, int B, int h, int w, int cin, int cout,
+                        const mk_resblock_params* params_host, int flags, float* out_dev, void* saved_dev,
+                        long long saved_bytes, void* ws_dev, long long ws_bytes, void* stream);
+int mk_resblock_backward(const void* saved_dev, const float* grad_out_dev, const long long* g_strides_host,
+                         const float* out_dev, int B, int h, int w, int cin, int cout, const mk_resblock_params* params_host,
+                         int flags, int want, const mk_resblock_grads* grads_host, void* ws_dev, long long ws_bytes,
+                         void* stream);
+
 /* (Re)seed the solver's device-side generator on `stream` (used in front of a CUDA-graph replay of mk_forward
  * captured with seed = 0). */
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream);
@@ -372,6 +427,24 @@ long long mk_op_sample_workspace_bytes(int B, int IM);
    maximising tr(R H) (det R = +1); H == 0 gives the identity, a NaN or +-inf anywhere in H gives nine NaNs.
    MK_ERR_INVALID for n < 0 or a null pointer. */
 int mk_op_kabsch(const double* H, double* R, int n, void* stream);
+
+/* The residual block's TF32 wgmma convolution GEMM alone, on caller buffers (padded NHWC geometry of B, h, w as in
+   mk_resblock_forward; R = B (h+2)(w+2), Rp = R rounded up to 4; taps 9 (3x3, padding 1) or 1 (1x1)):
+     mode 0 forward: a = X [R, cin] padded NHWC, b = W [cout, cin, taps]           -> out [R, cout]
+     mode 1 dgrad:   a = dZ [R, cout] padded NHWC, b = W [cout, cin, taps]         -> out [R, cin]
+     mode 2 wgrad:   a = dZ^T [cout, Rp], b = X^T [cin, Rp] (channel-major)        -> out = dW [cout, cin, taps]
+   W is rounded to TF32 on the way; a and b of mode 2 are used as given (the tensor core reads them as TF32).  Rows of the
+   pad ring in out are unspecified.  Workspace: mk_op_conv_tf32_ws_bytes bytes (-1 for bad arguments). */
+/* Byte offsets of the residual block's intermediates, for element-wise checks of each stage.  saved_off[6]: in the forward's
+   saved region, z1, z2 (pre-BN conv outputs, fp32 padded NHWC [R, cout]), a1 (BN1-apply + ReLU, TF32 padded NHWC),
+   a1^T (TF32 [cout, Rp]), x^T (TF32 [cin, Rp]), and the statistics mean1, rstd1, mean2, rstd2 (fp32 [4][cout]).  bwd_off[6]:
+   in the backward's workspace after a call, g = grad_out * mask (fp32 [R, cout]), dz (TF32 padded NHWC [R, cout]: dz1 when
+   the call computed dX or dW1/dBN1, else dz2), dz^T (TF32 [cout, Rp], the last BN backward's), dA1 (conv2's data gradient,
+   fp32 [R, cout]), conv1's and the shortcut's data gradients (fp32 [R, cin]). */
+int mk_resblock_layout(int B, int h, int w, int cin, int cout, long long* saved_off, long long* bwd_off);
+long long mk_op_conv_tf32_ws_bytes(int mode, int B, int h, int w, int cin, int cout, int taps);
+int mk_op_conv_tf32(int mode, const float* a, const float* b, float* out, int B, int h, int w, int cin, int cout, int taps,
+                    void* ws, long long ws_bytes, void* stream);
 
 #ifdef __cplusplus
 }

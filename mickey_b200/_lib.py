@@ -63,6 +63,16 @@ class MkHtrLayer(C.Structure):
 MkHtrLayerGrads = MkHtrLayer     # the same ten pointers, written instead of read
 
 
+class MkResblockParams(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("w1", "w2", "wsc", "bn1_w", "bn1_b", "bn1_mean", "bn1_var",
+                                          "bn2_w", "bn2_b", "bn2_mean", "bn2_var")] + \
+               [(n, C.c_float) for n in ("eps1", "eps2", "momentum1", "momentum2")]
+
+
+class MkResblockGrads(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("dx", "w1", "w2", "wsc", "bn1_w", "bn1_b", "bn2_w", "bn2_b")]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "mk_create": (C.c_int, [C.c_int, C.POINTER(MkConfig), C.POINTER(C.c_void_p)]),
@@ -132,6 +142,17 @@ EXPORTS = {
     "mk_head_transformer_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(MkHtrLayer),
                                                C.c_int, C.c_void_p, C.POINTER(MkHtrLayerGrads), C.c_void_p, C.c_longlong,
                                                C.c_void_p]),
+    "mk_resblock_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_resblock_saved_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_resblock_backward_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_resblock_forward": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.POINTER(MkResblockParams), C.c_int, C.c_void_p, C.c_void_p, C.c_longlong,
+                                      C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_resblock_layout": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_longlong),
+                                     C.POINTER(C.c_longlong)]),
+    "mk_resblock_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong), C.c_void_p, C.c_int, C.c_int,
+                                       C.c_int, C.c_int, C.c_int, C.POINTER(MkResblockParams), C.c_int, C.c_int,
+                                       C.POINTER(MkResblockGrads), C.c_void_p, C.c_longlong, C.c_void_p]),
     "mk_pose_to_submission": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "mk_launch_count": (C.c_longlong, [C.c_void_p]),
     "mk_pdl_enabled": (C.c_int, []),
@@ -152,6 +173,9 @@ EXPORTS = {
                                C.c_void_p, C.c_void_p, C.c_void_p]),
     "mk_op_sample_workspace_bytes": (C.c_longlong, [C.c_int, C.c_int]),
     "mk_op_kabsch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "mk_op_conv_tf32_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_op_conv_tf32": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                  C.c_int, C.c_void_p, C.c_longlong, C.c_void_p]),
 }
 
 _lib = None
