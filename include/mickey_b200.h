@@ -43,9 +43,9 @@ int mk_create(int device, const mk_config* cfg, mk_handle** out);
 int mk_destroy(mk_handle* h);
 const char* mk_last_error(void);
 const char* mk_version(void);
-/* sizeof(mk_config) / sizeof(mk_gemm_args) as compiled into the library (binding self-check). */
-int mk_sizeof_config(void);
-int mk_sizeof_gemm_args(void);
+/* sizeof the struct named `type` ("mk_config", "mk_gemm_args", ...) as compiled into the library, or -1 for a name it
+ * does not know (binding self-check). */
+int mk_sizeof(const char* type);
 
 /* Register a packed weight / table tensor that lives in device memory (replaces load_state_dict,
  * builder.py:11-13; the packing itself — fp16 cast, BatchNorm folding, per-head stacking — is done by

@@ -1,4 +1,5 @@
-"""ctypes binding of libmickey_b200.so (the C ABI declared in include/mickey_b200.h).
+"""ctypes binding of libmickey_b200.so (the C ABI declared in include/mickey_b200.h), and the rules every caller follows
+at that boundary: the stream argument, workspace allocation, the row pitch of N x N arguments and the handle's lifetime.
 
 There is no fallback: if the shared library is missing or does not load, importing the binding
 raises with the build command — the product path never routes around the CUDA extension.
@@ -6,7 +7,10 @@ raises with the build command — the product path never routes around the CUDA 
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", "libmickey_b200.so")
@@ -79,8 +83,7 @@ EXPORTS = {
     "mk_destroy": (C.c_int, [C.c_void_p]),
     "mk_last_error": (C.c_char_p, []),
     "mk_version": (C.c_char_p, []),
-    "mk_sizeof_config": (C.c_int, []),
-    "mk_sizeof_gemm_args": (C.c_int, []),
+    "mk_sizeof": (C.c_int, [C.c_char_p]),
     "mk_set_tensor": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.c_longlong]),
     "mk_finalize": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
     "mk_workspace_bytes": (C.c_longlong, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
@@ -178,6 +181,11 @@ EXPORTS = {
                                   C.c_int, C.c_void_p, C.c_longlong, C.c_void_p]),
 }
 
+# every struct the binding passes, by its C name: load() checks each size against the library's
+STRUCTS = {"mk_config": MkConfig, "mk_gemm_args": MkGemmArgs, "mk_htr_layer": MkHtrLayer,
+           "mk_htr_layer_grads": MkHtrLayerGrads, "mk_resblock_params": MkResblockParams,
+           "mk_resblock_grads": MkResblockGrads}
+
 _lib = None
 
 
@@ -199,10 +207,10 @@ def load():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args
-    if lib.mk_sizeof_config() != C.sizeof(MkConfig) or lib.mk_sizeof_gemm_args() != C.sizeof(MkGemmArgs):
-        raise MickeyB200Error("ctypes struct layout does not match the library (stale build?): "
-                              f"mk_config {lib.mk_sizeof_config()} vs {C.sizeof(MkConfig)}, "
-                              f"mk_gemm_args {lib.mk_sizeof_gemm_args()} vs {C.sizeof(MkGemmArgs)}")
+    sizes = {name: (lib.mk_sizeof(name.encode()), C.sizeof(st)) for name, st in STRUCTS.items()}
+    bad = [f"{name} {lib_size} vs {py_size}" for name, (lib_size, py_size) in sizes.items() if lib_size != py_size]
+    if bad:
+        raise MickeyB200Error("ctypes struct layout does not match the library (stale build?): " + ", ".join(bad))
     _lib = lib
     return lib
 
@@ -216,3 +224,62 @@ def check(rc: int, what: str = ""):
 def ptr(t):
     """Device (or host) address of a torch tensor, or None."""
     return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def stream(dev=None):
+    """The current CUDA stream of `dev` (None: the current device), as the library's `stream` argument."""
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def workspace(nbytes, dev, what: str):
+    """A uint8 buffer on `dev` for the byte count `nbytes` that the library's `what` (a mk_*_ws_bytes function) returned.
+    A negative count is the library rejecting the arguments, and raises; a zero count still gets one byte, so the
+    workspace pointer is never NULL."""
+    nbytes = int(nbytes)
+    if nbytes < 0:
+        raise MickeyB200Error(f"{what} returned {nbytes}: {load().mk_last_error().decode(errors='replace')}")
+    return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+
+
+def pitched(t):
+    """(tensor, row pitch in floats) for an fp32 [B, N, N] argument of the library.  t itself when its rows are contiguous,
+    at least N floats apart, and its matrices N row pitches apart (contiguous tensors, the engine's [B, N, pitch][:, :, :N]
+    views); any other layout (transposed, expanded, ...) becomes a contiguous copy with pitch N."""
+    B, N, _ = t.shape
+    s0, s1, s2 = t.stride()
+    if s2 == 1 and s1 >= N and (B == 1 or s0 == N * s1):
+        return t, s1
+    return t.contiguous(), N
+
+
+class Handle:
+    """An mk_handle of the library, created on `device` (a CUDA torch.device) for `cfg` (MkConfig) and destroyed with this
+    object: the tensors registered with it and the named buffers of its workspaces."""
+
+    def __init__(self, device, cfg: MkConfig):
+        self.lib = load()
+        self.device = device
+        h = C.c_void_p()
+        check(self.lib.mk_create(device.index or 0, C.byref(cfg), C.byref(h)), "mk_create")
+        self.h = h
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                self.lib.mk_destroy(self.h)
+        except Exception:
+            pass
+
+    def register(self, name: str, t):
+        """mk_set_tensor: the handle reads t (contiguous fp32 or fp16 on the handle's device) as `name` from now on."""
+        assert t.is_contiguous() and t.device == self.device
+        dt = {torch.float32: 0, torch.float16: 1}[t.dtype]
+        check(self.lib.mk_set_tensor(self.h, name.encode(), ptr(t), dt, t.numel()), f"mk_set_tensor({name})")
+
+    def workspace_view(self, ws, n_pairs: int, H: int, W: int, name: str, dtype, shape):
+        """Typed view of the named buffer of `ws`, a workspace laid out for n_pairs pairs of H x W images."""
+        off = self.lib.mk_workspace_offset(self.h, name.encode(), n_pairs, H, W)
+        if off < 0:
+            raise MickeyB200Error(self.lib.mk_last_error().decode())
+        nbytes = math.prod(shape) * torch.empty((), dtype=dtype).element_size()
+        return ws[off:off + nbytes].view(dtype).reshape(shape)

@@ -128,6 +128,16 @@ static inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 blo
     }                                                                                         \
   } while (0)
 
+#define MK_TRY(x) do { int rc_ = (x); if (rc_ != MK_OK) return rc_; } while (0)
+
 namespace mk {
 void set_last_error(const char* fmt, ...);
+
+// Row pitch (floats) of an fp32 [B, N, N] argument: <= 0 means contiguous (N).  A pitch below N would make rows overlap
+// and is rejected; `what` names the entry point and the argument in the message ("mk_match: nn_pitch").
+static inline int resolve_pitch(long long& pitch, int N, const char* what) {
+  if (pitch <= 0) pitch = N;
+  if (pitch < N) { set_last_error("%s %lld < N %d", what, pitch, N); return MK_ERR_INVALID; }
+  return MK_OK;
+}
 }

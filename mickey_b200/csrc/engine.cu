@@ -168,8 +168,6 @@ void set_conv_taps(GemmParams& p, int cin, int w2, bool three) {
   p.k_chunks = p.num_taps * p.chunks_per_tap;
 }
 
-#define MK_TRY(x) do { int rc_ = (x); if (rc_ != MK_OK) return rc_; } while (0)
-
 struct ProfScope {
   mk_handle* h; cudaStream_t st; int slot = -1;
   ProfScope(mk_handle* h_, const char* tag, cudaStream_t st_) : h(h_), st(st_) {
@@ -385,8 +383,7 @@ int run_match(mk_handle* h, int n_pairs, int N, float* scores, float* kp_scores,
     set_last_error("mk_match: final_scores is required; scores and kp_scores are given together or both NULL (lean mode)");
     return MK_ERR_INVALID;
   }
-  if (nn_pitch <= 0) nn_pitch = N;
-  if (nn_pitch < N) { set_last_error("mk_match: nn_pitch %lld < N %d", nn_pitch, N); return MK_ERR_INVALID; }
+  MK_TRY(resolve_pitch(nn_pitch, N, "mk_match: nn_pitch"));
   const bool tma_ok = nn_pitch % 4 == 0 && reinterpret_cast<uintptr_t>(final_scores) % 16 == 0 &&
                       (!scores || (reinterpret_cast<uintptr_t>(scores) % 16 == 0 && reinterpret_cast<uintptr_t>(kp_scores) % 16 == 0));
   const float inv_t = 1.0f / c.temperature;
@@ -419,7 +416,7 @@ int run_solve(mk_handle* h, const float* final_scores, long long nn_pitch, const
               Workspace& w, cudaStream_t st) {
   const mk_config& c = h->cfg;
   RansacParams rp{c.it_matches, c.it_ransac, c.num_sampled, c.num_corr, c.num_refine, c.th_inlier, c.th_soft_inlier, h->seed_dev};
-  if (nn_pitch <= 0) nn_pitch = N;
+  MK_TRY(resolve_pitch(nn_pitch, N, "mk_solve_pose: nn_pitch"));
   if (seed != 0) MK_TRY(seed_set(h->seed_dev, seed, st));      // seed == 0: continue the device-side sequence
   MK_CUDA_CHECK(cudaMemsetAsync(w.status, 0, (size_t)(SOLVER_COUNTER_BASE + n_pairs) * sizeof(int), st));
   const size_t n_idx = (size_t)n_pairs * c.it_matches * c.num_sampled;
@@ -469,8 +466,14 @@ extern "C" {
 
 const char* mk_last_error(void) { return mk::last_error(); }
 const char* mk_version(void) { return "mickey_b200 0.1.0 (sm_90a)"; }
-int mk_sizeof_config(void) { return (int)sizeof(mk_config); }
-int mk_sizeof_gemm_args(void) { return (int)sizeof(mk_gemm_args); }
+int mk_sizeof(const char* type) {
+  const std::unordered_map<std::string, int> sizes = {
+      {"mk_config", sizeof(mk_config)}, {"mk_gemm_args", sizeof(mk_gemm_args)}, {"mk_htr_layer", sizeof(mk_htr_layer)},
+      {"mk_htr_layer_grads", sizeof(mk_htr_layer_grads)}, {"mk_resblock_params", sizeof(mk_resblock_params)},
+      {"mk_resblock_grads", sizeof(mk_resblock_grads)}};
+  const auto it = type ? sizes.find(type) : sizes.end();
+  return it == sizes.end() ? -1 : it->second;
+}
 
 int mk_create(int device, const mk_config* cfg, mk_handle** out) {
   if (!cfg || !out) { set_last_error("null argument"); return MK_ERR_INVALID; }
@@ -820,7 +823,7 @@ int mk_op_matcher_reduce(const float* part_row, const float* part_col, const flo
 long long mk_op_sample_workspace_bytes(int B, int IM) { return (long long)sampler_workspace_bytes(B, IM) + 512; }
 int mk_op_sample(const float* fs, int B, int N, long long pitch, int IM, int n_sample, unsigned long long seed, void* ws,
                  long long ws_bytes, int* idx_out, int* status, void* stream) {
-  if (pitch <= 0) pitch = N;
+  MK_TRY(resolve_pitch(pitch, N, "mk_op_sample: pitch"));
   if ((long long)sampler_workspace_bytes(B, IM) + 256 > ws_bytes) { set_last_error("sampler workspace too small"); return MK_ERR_INVALID; }
   MK_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), (cudaStream_t)stream));
   // the seed word lives at the (256-byte aligned) end of the caller's workspace

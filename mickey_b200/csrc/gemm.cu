@@ -49,8 +49,6 @@ struct MapKeyHash {
 static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_map_cache;
 static std::mutex g_map_mutex;
 
-static int encode_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems,
-                                 int box_rows);
 static int encode_tensor_map_out_f16(CUtensorMap* map, const void* ptr, long long groups, long long rows, long long cols,
                                      int box_rows);
 
@@ -59,7 +57,7 @@ static int cached_map(const MapKey& key, CUtensorMap* map) {
   auto it = g_map_cache.find(key);
   if (it != g_map_cache.end()) { *map = it->second; return MK_OK; }
   int rc = key.groups ? encode_tensor_map_out_f16(map, key.ptr, key.groups, key.rows, key.cols, key.box)
-                      : encode_tensor_map_f16(map, key.ptr, key.rows, key.cols, key.ld, key.box);
+                      : encode_tensor_map_2d(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, key.ptr, key.rows, key.cols, key.ld, key.box);
   if (rc == MK_OK) {
     if (g_map_cache.size() > 4096) g_map_cache.clear();
     g_map_cache.emplace(key, *map);
@@ -76,19 +74,22 @@ int make_tensor_map_out_f16(CUtensorMap* map, void* ptr, long long groups, long 
   return cached_map(MapKey{ptr, rows, cols, cols, box_rows, groups}, map);
 }
 
-static int encode_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems,
-                                 int box_rows) {
+static_assert(BLOCK_K * 2 == 128, "an fp16 operand box is one 128-byte swizzle row wide");
+
+int encode_tensor_map_2d(CUtensorMap* map, CUtensorMapDataType dtype, const void* ptr, long long rows, long long cols,
+                         long long ld_elems, int box_rows) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) { set_last_error("cuTensorMapEncodeTiled entry point not available"); return MK_ERR_CUDA; }
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (ld_elems % 8)) {
-    set_last_error("tensor map operand must be 16-byte aligned with ld %% 8 == 0 (ptr=%p ld=%lld)", ptr, ld_elems);
+  const int esize = dtype == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : 2;
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (ld_elems * esize) % 16) {
+    set_last_error("tensor map operand must be 16-byte aligned with ld %% %d == 0 (ptr=%p ld=%lld)", 16 / esize, ptr, ld_elems);
     return MK_ERR_INVALID;
   }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld_elems * 2};
-  cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, (cuuint32_t)box_rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld_elems * esize};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = enc(map, dtype, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_last_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return MK_ERR_CUDA; }

@@ -12,6 +12,10 @@ struct GemmOperand {       // a row-major fp16 matrix [rows, cols] with leading 
 enum GemmImpl : int { GEMM_IMPL_DEFAULT = 0, GEMM_IMPL_TC = 1, GEMM_IMPL_SIMT = 2 };
 
 int make_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems, int box_rows);
+// Uncached TMA load map of a row-major fp16 or fp32 [rows, cols] operand with leading dimension ld_elems: box = 128 bytes
+// of columns x box_rows rows, 128-byte swizzle, zero fill.  The base and the row pitch must be 16-byte aligned.
+int encode_tensor_map_2d(CUtensorMap* map, CUtensorMapDataType dtype, const void* ptr, long long rows, long long cols,
+                         long long ld_elems, int box_rows);
 // TMA store map of a contiguous fp16 [groups, rows, cols] tensor (box 64 columns x box_rows rows, 128-byte swizzle)
 int make_tensor_map_out_f16(CUtensorMap* map, void* ptr, long long groups, long long rows, long long cols, int box_rows);
 int sm_count();            // SMs of the current device

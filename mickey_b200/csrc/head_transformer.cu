@@ -611,8 +611,6 @@ cudaError_t weight_grad(const float* A, long long lda, const float* Bm, long lon
 
 using namespace mk;
 
-#define HTR_CHECK(x) MK_CUDA_CHECK(x)
-
 long long mk_head_transformer_ws_bytes(int B, int h, int w, int num_layers, int save) {
   if (!geometry_ok(B, h, w, num_layers)) return -1;
   return (long long)fwd_layout(B, h * w, num_layers, save ? 1 : 0).total;
@@ -649,7 +647,7 @@ int mk_head_transformer(const float* x, const float* pe, int B, int h, int w, co
   float* xout = reinterpret_cast<float*>(base + F.xout);
   float* kvpart = reinterpret_cast<float*>(base + F.kvpart);
   float* wqkv = reinterpret_cast<float*>(base + F.wqkv);
-  HTR_CHECK(launch_k(htr_cm_to_tm_kernel, dim3(nch, B), dim3(256), 0, st, x, pe, N, w, at(0, F.layer.cat), D2));
+  MK_CUDA_CHECK(launch_k(htr_cm_to_tm_kernel, dim3(nch, B), dim3(256), 0, st, x, pe, N, w, at(0, F.layer.cat), D2));
   for (int l = 0; l < num_layers; ++l) {
     const mk_htr_layer& P = layers[l];
     float* cat = at(l, F.layer.cat);
@@ -657,22 +655,22 @@ int mk_head_transformer(const float* x, const float* pe, int B, int h, int w, co
     float* S = at(l, F.layer.S);
     float* msg = at(l, F.layer.msg);
     float* hb = at(l, F.layer.h);
-    HTR_CHECK(launch_k(htr_pack_qkv_kernel, dim3(48), dim3(256), 0, st, P.q_proj, P.k_proj, P.v_proj, wqkv));
-    HTR_CHECK((gemm<0, 0, HE_PHI>(gp(cat, D2, wqkv, D, T, D3, D, qkv, D3), 1, st)));
-    HTR_CHECK(launch_k(htr_kv_partial_kernel, dim3(nch, B), dim3(256), 0, st, (const float*)qkv, N, nch, kvpart));
-    HTR_CHECK(launch_k(htr_fold_kernel, dim3(ceil_div(SKV, 256), B), dim3(256), 0, st, (const float*)kvpart, nch, (long long)SKV,
+    MK_CUDA_CHECK(launch_k(htr_pack_qkv_kernel, dim3(48), dim3(256), 0, st, P.q_proj, P.k_proj, P.v_proj, wqkv));
+    MK_CUDA_CHECK((gemm<0, 0, HE_PHI>(gp(cat, D2, wqkv, D, T, D3, D, qkv, D3), 1, st)));
+    MK_CUDA_CHECK(launch_k(htr_kv_partial_kernel, dim3(nch, B), dim3(256), 0, st, (const float*)qkv, N, nch, kvpart));
+    MK_CUDA_CHECK(launch_k(htr_fold_kernel, dim3(ceil_div(SKV, 256), B), dim3(256), 0, st, (const float*)kvpart, nch, (long long)SKV,
                        (long long)nch * SKV, SKV, S, (long long)SKV));
-    HTR_CHECK(launch_k(htr_attn_fwd_kernel, dim3(nch, B), dim3(256), 0, st, (const float*)qkv, (const float*)S, N, msg));
+    MK_CUDA_CHECK(launch_k(htr_attn_fwd_kernel, dim3(nch, B), dim3(256), 0, st, (const float*)qkv, (const float*)S, N, msg));
     HGemm pm = gp(msg, D, P.merge, D, T, D, D, cat + D, D2);
     pm.gamma = P.norm1_w; pm.beta = P.norm1_b; pm.xhat = at(l, F.layer.xh1); pm.rstd = at(l, F.layer.rs1);
-    HTR_CHECK((gemm<0, 0, HE_LN>(pm, 1, st)));
-    HTR_CHECK((gemm<0, 0, HE_RELU>(gp(cat, D2, P.mlp0, D2, T, D2, D2, hb, D2), 1, st)));
+    MK_CUDA_CHECK((gemm<0, 0, HE_LN>(pm, 1, st)));
+    MK_CUDA_CHECK((gemm<0, 0, HE_RELU>(gp(cat, D2, P.mlp0, D2, T, D2, D2, hb, D2), 1, st)));
     const bool last = l + 1 == num_layers;
     HGemm p2 = gp(hb, D2, P.mlp2, D2, T, D, D2, last ? xout : at(l + 1, F.layer.cat), last ? D : D2);
     p2.R = cat; p2.ldr = D2; p2.gamma = P.norm2_w; p2.beta = P.norm2_b; p2.xhat = at(l, F.layer.xh2); p2.rstd = at(l, F.layer.rs2);
-    HTR_CHECK((gemm<0, 0, HE_LN_RES>(p2, 1, st)));
+    MK_CUDA_CHECK((gemm<0, 0, HE_LN_RES>(p2, 1, st)));
   }
-  HTR_CHECK(launch_k(htr_tm_to_cm_kernel, dim3(nch, B), dim3(256), 0, st, (const float*)xout, D, N, out));
+  MK_CUDA_CHECK(launch_k(htr_tm_to_cm_kernel, dim3(nch, B), dim3(256), 0, st, (const float*)xout, D, N, out));
   return MK_OK;
 }
 
@@ -723,55 +721,55 @@ int mk_head_transformer_backward(const void* saved, const float* grad_out, int B
       e = launch_k(htr_fold_kernel, dim3(1, 1), dim3(256), 0, st, (const float*)(lnpart + D), nln, (long long)2 * D, 0LL, D, dbeta, 0LL);
     return e;
   };
-  HTR_CHECK(launch_k(htr_cm_to_tm_kernel, dim3(nch, B), dim3(256), 0, st, grad_out, (const float*)nullptr, N, w, g, D));
+  MK_CUDA_CHECK(launch_k(htr_cm_to_tm_kernel, dim3(nch, B), dim3(256), 0, st, grad_out, (const float*)nullptr, N, w, g, D));
   for (int l = num_layers - 1; l >= 0; --l) {
     const mk_htr_layer& P = layers[l];
     const mk_htr_layer_grads& G = grads[l];
     const float *cat = at(l, F.layer.cat), *qkv = at(l, F.layer.qkv), *msg = at(l, F.layer.msg), *hb = at(l, F.layer.h);
     // norm2, mlp.2
-    HTR_CHECK(launch_k(htr_ln_bwd_kernel, dim3(nln), dim3(256), 0, st, (const float*)g, at(l, F.layer.xh2), at(l, F.layer.rs2),
+    MK_CUDA_CHECK(launch_k(htr_ln_bwd_kernel, dim3(nln), dim3(256), 0, st, (const float*)g, at(l, F.layer.xh2), at(l, F.layer.rs2),
                        P.norm2_w, T, dy, lnpart));
-    HTR_CHECK(ln_fold(G.norm2_w, G.norm2_b));
-    if (G.mlp2) HTR_CHECK(weight_grad(dy, D, hb, D2, D, D2, T, wpart, G.mlp2, st));
+    MK_CUDA_CHECK(ln_fold(G.norm2_w, G.norm2_b));
+    if (G.mlp2) MK_CUDA_CHECK(weight_grad(dy, D, hb, D2, D, D2, T, wpart, G.mlp2, st));
     const bool rest = need_below(l) || G.mlp0 || G.merge || G.norm1_w || G.norm1_b || G.q_proj || G.k_proj || G.v_proj;
     if (!rest) break;
     // ReLU, mlp.0: dcat = dh W0; its x half joins the residual path, its m1 half goes to norm1
     {
       HGemm p = gp(dy, D, P.mlp2, D2, T, D2, D, dh, D2);
       p.R = hb; p.ldr = D2;
-      HTR_CHECK((gemm<0, 1, HE_MASK>(p, 1, st)));
+      MK_CUDA_CHECK((gemm<0, 1, HE_MASK>(p, 1, st)));
     }
-    if (G.mlp0) HTR_CHECK(weight_grad(dh, D2, cat, D2, D2, D2, T, wpart, G.mlp0, st));
+    if (G.mlp0) MK_CUDA_CHECK(weight_grad(dh, D2, cat, D2, D2, D2, T, wpart, G.mlp0, st));
     if (need_below(l)) {
       HGemm p = gp(dh, D2, P.mlp0, D2, T, D, D2, gn, D);
       p.R = g; p.ldr = D;
-      HTR_CHECK((gemm<0, 1, HE_ADD>(p, 1, st)));
+      MK_CUDA_CHECK((gemm<0, 1, HE_ADD>(p, 1, st)));
     }
-    HTR_CHECK((gemm<0, 1, HE_STORE>(gp(dh, D2, P.mlp0 + D, D2, T, D, D2, dm, D), 1, st)));
+    MK_CUDA_CHECK((gemm<0, 1, HE_STORE>(gp(dh, D2, P.mlp0 + D, D2, T, D, D2, dm, D), 1, st)));
     // norm1, merge
-    HTR_CHECK(launch_k(htr_ln_bwd_kernel, dim3(nln), dim3(256), 0, st, (const float*)dm, at(l, F.layer.xh1), at(l, F.layer.rs1),
+    MK_CUDA_CHECK(launch_k(htr_ln_bwd_kernel, dim3(nln), dim3(256), 0, st, (const float*)dm, at(l, F.layer.xh1), at(l, F.layer.rs1),
                        P.norm1_w, T, dy, lnpart));
-    HTR_CHECK(ln_fold(G.norm1_w, G.norm1_b));
-    if (G.merge) HTR_CHECK(weight_grad(dy, D, msg, D, D, D, T, wpart, G.merge, st));
-    HTR_CHECK((gemm<0, 1, HE_STORE>(gp(dy, D, P.merge, D, T, D, D, dm, D), 1, st)));
+    MK_CUDA_CHECK(ln_fold(G.norm1_w, G.norm1_b));
+    if (G.merge) MK_CUDA_CHECK(weight_grad(dy, D, msg, D, D, D, T, wpart, G.merge, st));
+    MK_CUDA_CHECK((gemm<0, 1, HE_STORE>(gp(dy, D, P.merge, D, T, D, D, dm, D), 1, st)));
     // linear attention
-    HTR_CHECK(launch_k(htr_attn_bwd_q_kernel, dim3(nch, B), dim3(256), 0, st, qkv, at(l, F.layer.S), (const float*)dm, N, nch,
+    MK_CUDA_CHECK(launch_k(htr_attn_bwd_q_kernel, dim3(nch, B), dim3(256), 0, st, qkv, at(l, F.layer.S), (const float*)dm, N, nch,
                        dqkv, apart));
-    HTR_CHECK(launch_k(htr_fold_kernel, dim3(ceil_div(SKV, 256), B), dim3(256), 0, st, (const float*)apart, nch, (long long)SKV,
+    MK_CUDA_CHECK(launch_k(htr_fold_kernel, dim3(ceil_div(SKV, 256), B), dim3(256), 0, st, (const float*)apart, nch, (long long)SKV,
                        (long long)nch * SKV, SKV, dS, (long long)SKV));
-    HTR_CHECK(launch_k(htr_attn_bwd_kv_kernel, dim3(nch, B), dim3(256), 0, st, qkv, (const float*)dS, N, dqkv));
+    MK_CUDA_CHECK(launch_k(htr_attn_bwd_kv_kernel, dim3(nch, B), dim3(256), 0, st, qkv, (const float*)dS, N, dqkv));
     float* wg[3] = {G.q_proj, G.k_proj, G.v_proj};
     for (int i = 0; i < 3; ++i)
-      if (wg[i]) HTR_CHECK(weight_grad(dqkv + i * D, D3, cat, D2, D, D, T, wpart, wg[i], st));
+      if (wg[i]) MK_CUDA_CHECK(weight_grad(dqkv + i * D, D3, cat, D2, D, D, T, wpart, wg[i], st));
     if (!need_below(l)) break;
-    HTR_CHECK(launch_k(htr_pack_qkv_kernel, dim3(48), dim3(256), 0, st, P.q_proj, P.k_proj, P.v_proj, wqkv));
+    MK_CUDA_CHECK(launch_k(htr_pack_qkv_kernel, dim3(48), dim3(256), 0, st, P.q_proj, P.k_proj, P.v_proj, wqkv));
     {
       HGemm p = gp(dqkv, D3, wqkv, D, T, D, D3, gn, D);
       p.R = gn; p.ldr = D;
-      HTR_CHECK((gemm<0, 1, HE_ADD>(p, 1, st)));
+      MK_CUDA_CHECK((gemm<0, 1, HE_ADD>(p, 1, st)));
     }
     float* t = g; g = gn; gn = t;
   }
-  if (grad_x) HTR_CHECK(launch_k(htr_tm_to_cm_kernel, dim3(nch, B), dim3(256), 0, st, (const float*)g, D, N, grad_x));
+  if (grad_x) MK_CUDA_CHECK(launch_k(htr_tm_to_cm_kernel, dim3(nch, B), dim3(256), 0, st, (const float*)g, D, N, grad_x));
   return MK_OK;
 }

@@ -251,9 +251,9 @@ int loss_search(const float* fs, long long pitch, const float* kps0, const float
                 const float* K0, const float* K1, int B, int N, int IM, int IR, int S, int C, int n_ref, float th_ref,
                 unsigned long long seed, const int* outer_idx, const int* inner_idx, int* sampled_out, int* inner_out,
                 uint32_t* inl_out, int* status, void* ws, long long ws_bytes, cudaStream_t st) {
-  if (pitch <= 0) pitch = N;
+  MK_TRY(resolve_pitch(pitch, N, "mk_loss_search: pitch"));
   if (!fs || !kps0 || !d0 || !kps1 || !d1 || !K0 || !K1 || !sampled_out || !inner_out || !inl_out || !status || !ws || B <= 0 ||
-      N <= 0 || pitch < N || IM <= 0 || IR <= 0 || n_ref < 0 || S <= 0 || S % 32 || S > LOSS_MAX_S || C < 1 ||
+      N <= 0 || IM <= 0 || IR <= 0 || n_ref < 0 || S <= 0 || S % 32 || S > LOSS_MAX_S || C < 1 ||
       C > LOSS_MAX_C || C > S || (long long)N * N < S || (long long)N * N > 0x7fffffffLL || !(th_ref == th_ref)) {
     // S % 32: the inlier masks are whole 32-bit words, one bit per set entry
     set_last_error("mk_loss_search: need non-NULL inputs, outputs, status and workspace, B, N, IM, IR > 0, pitch >= N, "

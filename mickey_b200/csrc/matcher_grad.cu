@@ -411,8 +411,7 @@ int mk_dual_softmax(const float* dsc0, const float* dsc1, const float* scr0, con
                    "alone, or scores alone");
     return MK_ERR_INVALID;
   }
-  if (nn_pitch <= 0) nn_pitch = N;
-  if (nn_pitch < N) { set_last_error("mk_dual_softmax: nn_pitch %lld < N %d", nn_pitch, N); return MK_ERR_INVALID; }
+  MK_TRY(resolve_pitch(nn_pitch, N, "mk_dual_softmax: nn_pitch"));
   const FwdLayout L = fwd_layout(B, N);
   if (ws_bytes < (long long)L.total) {
     set_last_error("mk_dual_softmax: workspace of %lld bytes, %lld needed", ws_bytes, (long long)L.total);
@@ -475,11 +474,7 @@ int mk_dual_softmax_backward(const float* dsc0, const float* dsc1, const float* 
     return MK_ERR_INVALID;
   }
   if (dustbin && !ddustbin) { set_last_error("mk_dual_softmax_backward: the dustbin needs ddustbin"); return MK_ERR_INVALID; }
-  long long* pitch[3] = {&gs_pitch, &gk_pitch, &gf_pitch};
-  for (long long* pp : pitch) {
-    if (*pp <= 0) *pp = N;
-    if (*pp < N) { set_last_error("mk_dual_softmax_backward: gradient pitch %lld < N %d", *pp, N); return MK_ERR_INVALID; }
-  }
+  for (long long* pp : {&gs_pitch, &gk_pitch, &gf_pitch}) MK_TRY(resolve_pitch(*pp, N, "mk_dual_softmax_backward: gradient pitch"));
   const BwdLayout L = bwd_layout(B, N);
   if (ws_bytes < (long long)L.total) {
     set_last_error("mk_dual_softmax_backward: workspace of %lld bytes, %lld needed", ws_bytes, (long long)L.total);

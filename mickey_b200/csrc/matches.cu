@@ -199,9 +199,9 @@ long long mutual_matches_ws_bytes(int B, int N) {
 
 int mutual_matches(const float* scores, long long pitch, int B, int N, float min_conf, int* matches, float* match_scores,
                    int* count, void* ws, long long ws_bytes, cudaStream_t s) {
-  if (pitch <= 0) pitch = N;
-  if (!scores || !matches || !match_scores || !count || !ws || B <= 0 || N < 2 || N - 1 > MAX_SORT || pitch < N ||
-      isnan(min_conf) || isinf(min_conf)) {
+  MK_TRY(resolve_pitch(pitch, N, "mk_mutual_matches: nn_pitch"));
+  if (!scores || !matches || !match_scores || !count || !ws || B <= 0 || N < 2 || N - 1 > MAX_SORT || isnan(min_conf) ||
+      isinf(min_conf)) {
     set_last_error("mk_mutual_matches: need non-NULL scores / matches / match_scores / count / workspace, B > 0, "
                    "2 <= N <= %d, pitch >= N and a finite min_conf (got B %d, N %d, pitch %lld, min_conf %g)",
                    MAX_SORT + 1, B, N, pitch, (double)min_conf);

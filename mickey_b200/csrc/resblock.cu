@@ -20,10 +20,11 @@
 // second moment), and running statistics are updated as F.batch_norm does.  No atomics anywhere: every output, gradient
 // and running statistic is bit-identical run to run.
 #include "../../include/mickey_b200.h"
+#include "gemm.h"
 #include "gemm_tc.cuh"
 
+#include <algorithm>
 #include <cstring>
-#include <mutex>
 
 namespace mk {
 
@@ -476,36 +477,7 @@ __global__ void __launch_bounds__(256) rb_wfold_kernel(const float* part, int sl
 }
 
 // ---- host side ----------------------------------------------------------------------------------------------------
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-PFN_encodeTiled encoder() {
-  static PFN_encodeTiled fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_encodeTiled>(p);
-  });
-  return fn;
-}
-
-// fp32 [rows, cols] with row pitch ld floats; box = 32 columns (128 bytes) x box_rows, 128-byte swizzle, zero fill
-int tmap_f32(CUtensorMap* m, const float* ptr, long long rows, long long cols, long long ld, int box_rows) {
-  PFN_encodeTiled enc = encoder();
-  if (!enc) { set_last_error("cuTensorMapEncodeTiled entry point not available"); return MK_ERR_CUDA; }
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t box[2] = {(cuuint32_t)RB_BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_last_error("cuTensorMapEncodeTiled (fp32) failed with CUresult %d", (int)r); return MK_ERR_CUDA; }
-  return MK_OK;
-}
+static_assert(RB_BK * 4 == 128, "encode_tensor_map_2d's fp32 box is one 128-byte swizzle row: RB_BK columns");
 
 size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
@@ -544,18 +516,12 @@ cudaError_t launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const RbGemm
   return launch_k(rb_gemm_kernel<BN, WGRAD>, grid, dim3(RB_THREADS), smem, st, a, b, p);
 }
 
-#define RB_TRY(x)                          \
-  do {                                     \
-    const int rc_ = (x);                   \
-    if (rc_ != MK_OK) return rc_;          \
-  } while (0)
-
 // forward / dgrad: out [R, N] = sum_t A[r + shift(t)] . Bw[n, t, :]; A [R, K1] (K1 = channels), Bw [N, taps K1]
 int conv_fwd(const Geo& g, const float* A, int K1, const float* Bw, int N, int taps, float* out, cudaStream_t st) {
   CUtensorMap ta, tb;
-  RB_TRY(tmap_f32(&ta, A, g.R, K1, K1, RB_BM));
+  MK_TRY(encode_tensor_map_2d(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, A, g.R, K1, K1, RB_BM));
   const int bn = bn_of(N);
-  RB_TRY(tmap_f32(&tb, Bw, N, (long long)taps * K1, (long long)taps * K1, bn));
+  MK_TRY(encode_tensor_map_2d(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, Bw, N, (long long)taps * K1, (long long)taps * K1, bn));
   RbGemm p;
   memset(&p, 0, sizeof(p));
   p.M = g.R; p.N = N; p.cpt = K1 / RB_BK; p.k_chunks = taps * p.cpt; p.taps = taps;
@@ -576,7 +542,7 @@ int conv_wgrad(const Geo& g, const float* dZT, const float* XT, int cout, int ci
   int shift[9];
   conv_shifts(g, taps, shift);
   CUtensorMap ta, tb;
-  RB_TRY(tmap_f32(&ta, dZT, cout, g.Rp, g.Rp, RB_BM));
+  MK_TRY(encode_tensor_map_2d(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dZT, cout, g.Rp, g.Rp, RB_BM));
   RbGemm p;
   memset(&p, 0, sizeof(p));
   p.M = cout; p.N = cin; p.k_chunks = ceil_div(g.R, RB_BK); p.taps = 1; p.cin = cin; p.chunks_per_slot = cps;
@@ -589,7 +555,7 @@ int conv_wgrad(const Geo& g, const float* dZT, const float* XT, int cout, int ci
       MK_CUDA_CHECK(launch_k(rb_shift_kernel, dim3((unsigned)((n_op + 255) / 256)), dim3(256), 0, st, XT, xs, cin, g.Rp, shift[t]));
       B = xs;
     }
-    RB_TRY(tmap_f32(&tb, B, cin, g.Rp, g.Rp, bn));
+    MK_TRY(encode_tensor_map_2d(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, B, cin, g.Rp, g.Rp, bn));
     p.out = part + (long long)t * cin;
     MK_CUDA_CHECK((bn == 128 ? launch_gemm<128, true>(ta, tb, p, grid, st) : launch_gemm<64, true>(ta, tb, p, grid, st)));
   }
@@ -767,11 +733,11 @@ int mk_resblock_forward(const float* x, const long long* x_strides, int B, int h
     Pack k;
     memset(&k, 0, sizeof(k));
     k.C = cin; k.src = xin; k.o_tf = xp; k.o_cm = save ? xT : nullptr;
-    RB_TRY(pack<PK_NCHW>(g, k, st));
+    MK_TRY(pack<PK_NCHW>(g, k, st));
   }
-  RB_TRY(relayout(P->w1, cout, cin, 9, 0, F(L.wk1), st));
-  RB_TRY(relayout(P->w2, cout, cout, 9, 0, F(L.wk2), st));
-  if (P->wsc) RB_TRY(relayout(P->wsc, cout, cin, 1, 0, F(L.wksc), st));
+  MK_TRY(relayout(P->w1, cout, cin, 9, 0, F(L.wk1), st));
+  MK_TRY(relayout(P->w2, cout, cout, 9, 0, F(L.wk2), st));
+  if (P->wsc) MK_TRY(relayout(P->wsc, cout, cin, 1, 0, F(L.wksc), st));
 
   auto bn_stats = [&](const float* Z, const float* gamma, float* mean, float* rstd, float* rm, float* rv, float eps,
                       float mom) -> int {
@@ -783,27 +749,27 @@ int mk_resblock_forward(const float* x, const long long* x_strides, int B, int h
     Stats s;
     memset(&s, 0, sizeof(s));
     s.C = cout; s.rows_per_slot = ceil_div(g.R, f.slots); s.G = Z; s.part = spart;
-    RB_TRY(stats(g, s, st));
-    RB_TRY(fold(FD_MEAN, f, st));
+    MK_TRY(stats(g, s, st));
+    MK_TRY(fold(FD_MEAN, f, st));
     s.shift = mean;
-    RB_TRY(stats(g, s, st));
+    MK_TRY(stats(g, s, st));
     return fold(FD_VAR, f, st);
   };
 
   // conv1 -> BN1 -> ReLU
-  RB_TRY(conv_fwd(g, xp, cin, F(L.wk1), cout, 9, z1, st));
-  if (bn) RB_TRY(bn_stats(z1, P->bn1_w, mean1, rstd1, P->bn1_mean, P->bn1_var, P->eps1, P->momentum1));
+  MK_TRY(conv_fwd(g, xp, cin, F(L.wk1), cout, 9, z1, st));
+  if (bn) MK_TRY(bn_stats(z1, P->bn1_w, mean1, rstd1, P->bn1_mean, P->bn1_var, P->eps1, P->momentum1));
   {
     Pack k;
     memset(&k, 0, sizeof(k));
     k.C = cout; k.Z = z1; k.bn = bn; k.mean = mean1; k.rstd = rstd1; k.gamma = P->bn1_w; k.beta = P->bn1_b;
     k.o_tf = a1; k.o_cm = save ? a1T : nullptr;
-    RB_TRY(pack<PK_BN_FWD>(g, k, st));
+    MK_TRY(pack<PK_BN_FWD>(g, k, st));
   }
   // conv2 -> BN2, shortcut, add, ReLU
-  RB_TRY(conv_fwd(g, a1, cout, F(L.wk2), cout, 9, z2, st));
-  if (bn) RB_TRY(bn_stats(z2, P->bn2_w, mean2, rstd2, P->bn2_mean, P->bn2_var, P->eps2, P->momentum2));
-  if (P->wsc) RB_TRY(conv_fwd(g, xp, cin, F(L.wksc), cout, 1, sc, st));
+  MK_TRY(conv_fwd(g, a1, cout, F(L.wk2), cout, 9, z2, st));
+  if (bn) MK_TRY(bn_stats(z2, P->bn2_w, mean2, rstd2, P->bn2_mean, P->bn2_var, P->eps2, P->momentum2));
+  if (P->wsc) MK_TRY(conv_fwd(g, xp, cin, F(L.wksc), cout, 1, sc, st));
   Final k;
   memset(&k, 0, sizeof(k));
   k.C = cout; k.bn = bn; k.relu = relu; k.Z = z2; k.mean = mean2; k.rstd = rstd2; k.gamma = P->bn2_w; k.beta = P->bn2_b;
@@ -871,13 +837,13 @@ int mk_resblock_backward(const void* saved, const float* grad_out, const long lo
     k.o_f32 = gf;
     if (sc && want_dx) k.o_tf = gr;
     if (sc && (want & MK_RB_GRAD_WSC)) k.o_cm = grT;
-    RB_TRY(pack<PK_NCHW>(g, k, st));
+    MK_TRY(pack<PK_NCHW>(g, k, st));
   }
   // 2. the shortcut's wgrad and dgrad
-  if (sc && (want & MK_RB_GRAD_WSC)) RB_TRY(conv_wgrad(g, grT, xT, cout, cin, 1, xs, wpart, G->wsc, st));
+  if (sc && (want & MK_RB_GRAD_WSC)) MK_TRY(conv_wgrad(g, grT, xT, cout, cin, 1, xs, wpart, G->wsc, st));
   if (sc && want_dx) {
-    RB_TRY(relayout(P->wsc, cout, cin, 1, 1, F(L.wdsc), st));
-    RB_TRY(conv_fwd(g, gr, cout, F(L.wdsc), cin, 1, dxs, st));
+    MK_TRY(relayout(P->wsc, cout, cin, 1, 1, F(L.wdsc), st));
+    MK_TRY(conv_fwd(g, gr, cout, F(L.wdsc), cin, 1, dxs, st));
   }
   // BN backward: sums of g and g xhat, then dz = gamma rstd / M (M g - sum g - xhat sum g xhat), TF32 in both layouts
   auto bn_bwd = [&](const float* Gin, const float* Mk, const float* Z, const float* mean, const float* rstd, const float* gamma,
@@ -891,33 +857,33 @@ int mk_resblock_backward(const void* saved, const float* grad_out, const long lo
       memset(&s, 0, sizeof(s));
       s.C = cout; s.rows_per_slot = ceil_div(g.R, stat_slots(g)); s.G = Gin; s.Mk = Mk; s.Zx = Z; s.mean = mean; s.rstd = rstd;
       s.part = spart;
-      RB_TRY(stats(g, s, st));
+      MK_TRY(stats(g, s, st));
       Fold f;
       memset(&f, 0, sizeof(f));
       f.C = cout; f.slots = stat_slots(g); f.train = train; f.count = count; f.part = spart; f.rstd = const_cast<float*>(rstd);
       f.gamma = gamma; f.dgamma = dgamma; f.dbeta = dbeta; f.coef = coef;
-      RB_TRY(fold(FD_BWD, f, st));
+      MK_TRY(fold(FD_BWD, f, st));
     }
     if (!need_nhwc && !need_cm) return MK_OK;
     return pack<PK_BN_BWD>(g, k, st);
   };
   // 3. BN2 backward
   if (below_bn2 || (want & (MK_RB_GRAD_BN2_W | MK_RB_GRAD_BN2_B)))
-    RB_TRY(bn_bwd(gf, nullptr, z2, mean2, rstd2, P->bn2_w, (want & MK_RB_GRAD_BN2_W) ? G->bn2_w : nullptr,
+    MK_TRY(bn_bwd(gf, nullptr, z2, mean2, rstd2, P->bn2_w, (want & MK_RB_GRAD_BN2_W) ? G->bn2_w : nullptr,
                   (want & MK_RB_GRAD_BN2_B) ? G->bn2_b : nullptr, below2, want & MK_RB_GRAD_W2));
   // 4. conv2's wgrad and dgrad
-  if (want & MK_RB_GRAD_W2) RB_TRY(conv_wgrad(g, dzT, a1T, cout, cout, 9, xs, wpart, G->w2, st));
+  if (want & MK_RB_GRAD_W2) MK_TRY(conv_wgrad(g, dzT, a1T, cout, cout, 9, xs, wpart, G->w2, st));
   if (below2) {
-    RB_TRY(relayout(P->w2, cout, cout, 9, 1, wd, st));
-    RB_TRY(conv_fwd(g, dz, cout, wd, cout, 9, da1, st));
+    MK_TRY(relayout(P->w2, cout, cout, 9, 1, wd, st));
+    MK_TRY(conv_fwd(g, dz, cout, wd, cout, 9, da1, st));
     // 5-6. the ReLU1 mask and BN1 backward
-    RB_TRY(bn_bwd(da1, a1, z1, mean1, rstd1, P->bn1_w, (want & MK_RB_GRAD_BN1_W) ? G->bn1_w : nullptr,
+    MK_TRY(bn_bwd(da1, a1, z1, mean1, rstd1, P->bn1_w, (want & MK_RB_GRAD_BN1_W) ? G->bn1_w : nullptr,
                   (want & MK_RB_GRAD_BN1_B) ? G->bn1_b : nullptr, want_dx, want & MK_RB_GRAD_W1));
     // 7. conv1's wgrad, and its dgrad only for dX
-    if (want & MK_RB_GRAD_W1) RB_TRY(conv_wgrad(g, dzT, xT, cout, cin, 9, xs, wpart, G->w1, st));
+    if (want & MK_RB_GRAD_W1) MK_TRY(conv_wgrad(g, dzT, xT, cout, cin, 9, xs, wpart, G->w1, st));
     if (want_dx) {
-      RB_TRY(relayout(P->w1, cout, cin, 9, 1, wd, st));
-      RB_TRY(conv_fwd(g, dz, cout, wd, cin, 9, dxc, st));
+      MK_TRY(relayout(P->w1, cout, cin, 9, 1, wd, st));
+      MK_TRY(conv_fwd(g, dz, cout, wd, cin, 9, dxc, st));
     }
   }
   // 8. dX = conv1's data gradient + the shortcut's
@@ -949,11 +915,11 @@ int mk_op_conv_tf32(int mode, const float* a, const float* b, float* out, int B,
   cudaStream_t st = (cudaStream_t)stream;
   float* wk = reinterpret_cast<float*>(ws);
   if (mode == 0) {             // out [R, cout] = conv(a [R, cin] padded NHWC, b = W [cout, cin, taps])
-    RB_TRY(relayout(b, cout, cin, taps, 0, wk, st));
+    MK_TRY(relayout(b, cout, cin, taps, 0, wk, st));
     return conv_fwd(g, a, cin, wk, cout, taps, out, st);
   }
   if (mode == 1) {             // out [R, cin] = dgrad(a = dZ [R, cout] padded NHWC, b = W [cout, cin, taps])
-    RB_TRY(relayout(b, cout, cin, taps, 1, wk, st));
+    MK_TRY(relayout(b, cout, cin, taps, 1, wk, st));
     return conv_fwd(g, a, cout, wk, cin, taps, out, st);
   }
   // out = dW [cout, cin, taps] from a = dZ^T [cout, Rp], b = X^T [cin, Rp]

@@ -9,7 +9,6 @@ layout the extractor turns into the heads' input.  INTEGRATION.md shows the swap
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, Optional
 
 import torch
@@ -17,7 +16,7 @@ import torch.nn as nn
 
 from . import _lib
 from .config import VARIANTS
-from .engine import PATCH, interpolate_pos_embed, pack_backbone
+from .engine import PATCH, pack_backbone, position_tables, raw_positions
 
 POS_GRID = 37               # img_size 518 / patch 14 (mickey_extractor.py:18-22)
 MIN_SIDE = 7 * PATCH        # the smallest image the engine accepts
@@ -48,42 +47,26 @@ class _Block(nn.Module):
         self.ls2 = _Params(gamma=(D,))
 
 
-class _Packed:
+class _Packed(_lib.Handle):
     """The C handle, the packed weights, the per-geometry tables and the workspace of one device.  Kept in the module's
     __dict__, outside the state dict."""
 
     def __init__(self, module: "DinoVisionTransformer", device: torch.device):
-        self.lib = _lib.load()
-        self.device = device
         D, depth, heads = VARIANTS[module.variant]
         cfg = _lib.MkConfig()
         cfg.embed_dim, cfg.depth, cfg.heads, cfg.down_factor = D, depth, heads, PATCH
-        h = C.c_void_p()
-        _lib.check(self.lib.mk_create(device.index or 0, C.byref(cfg), C.byref(h)), "mk_create")
-        self.h = h
+        super().__init__(device, cfg)
         with torch.no_grad():
             sd = dict(module.named_parameters())
             self.packed = pack_backbone(sd, module.variant, device, prefix="")
-            self.raw_pos = (sd["pos_embed"].detach().float(), sd["cls_token"].detach().float(),
-                            sd["patch_embed.proj.bias"].detach().float())
+            self.raw_pos = raw_positions(sd, device, prefix="")
         for name, t in self.packed.items():
-            self._register(name, t)
+            self.register(name, t)
         self.tables: Dict[tuple, Dict[str, torch.Tensor]] = {}
         self.geo = None
         self.ws = None
         self.n_img = 0
         self.stream = torch.cuda.current_stream(device)
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                self.lib.mk_destroy(self.h)
-        except Exception:
-            pass
-
-    def _register(self, name, t):
-        dt = {torch.float32: 0, torch.float16: 1}[t.dtype]
-        _lib.check(self.lib.mk_set_tensor(self.h, name.encode(), _lib.ptr(t), dt, t.numel()), f"mk_set_tensor({name})")
 
     def buffers(self):
         yield from self.packed.values()
@@ -106,27 +89,20 @@ class _Packed:
             return
         tb = self.tables.get((H, W))
         if tb is None:
-            gh, gw = H // PATCH, W // PATCH
-            pos, cls, pbias = self.raw_pos
-            with torch.no_grad():
-                full = interpolate_pos_embed(pos, gh, gw)
-                tb = {"patch.posb": (full[1:] + pbias[None]).contiguous(),
-                      "patch.clspos": (cls.reshape(-1) + full[0]).contiguous()}
+            tb = position_tables(self.raw_pos, H, W)
             if len(self.tables) >= MAX_GEOMETRIES:
                 del self.tables[next(iter(self.tables))]
             self.tables[(H, W)] = tb
         for n, t in tb.items():
-            self._register(n, t)
+            self.register(n, t)
         _lib.check(self.lib.mk_finalize(self.h, H, W), "mk_finalize")
         self.geo = (H, W)
 
     def workspace(self, n_img, H, W):
         nbytes = int(self.lib.mk_backbone_ws_bytes(self.h, n_img, H, W))
-        if nbytes < 0:
-            raise _lib.MickeyB200Error(f"mk_backbone_ws_bytes({n_img}, {H}, {W}) failed")
-        if self.ws is None or self.ws.numel() < nbytes:
+        if self.ws is None or not 0 <= nbytes <= self.ws.numel():
             self.ws = None
-            self.ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            self.ws = _lib.workspace(nbytes, self.device, f"mk_backbone_ws_bytes({n_img}, {H}, {W})")
         return self.ws
 
 
@@ -215,14 +191,13 @@ class DinoVisionTransformer(nn.Module):
         N = (H // PATCH) * (W // PATCH)
         with torch.cuda.device(dev), torch.no_grad():
             st = self._state(dev)
-            stream = torch.cuda.current_stream(dev)
-            st.on_stream(stream)
+            st.on_stream(torch.cuda.current_stream(dev))
             st.use_geometry(H, W)
             ws = st.workspace(B, H, W)
             images = x.to(torch.float32, memory_format=torch.contiguous_format)
             out = torch.empty(B, D, N, dtype=torch.float32, device=dev)
             _lib.check(st.lib.mk_backbone_features(st.h, _lib.ptr(images), B, H, W, _lib.ptr(out), _lib.ptr(ws),
-                                                   ws.numel(), C.c_void_p(stream.cuda_stream)), "mk_backbone_features")
+                                                   ws.numel(), _lib.stream(dev)), "mk_backbone_features")
             st.n_img = B
         return {"x_norm_patchtokens": out.permute(0, 2, 1)}
 
@@ -236,11 +211,4 @@ class DinoVisionTransformer(nn.Module):
         if st is None or st.geo is None or st.n_img % 2:
             raise _lib.MickeyB200Error("ws_view needs a previous forward_features call on an even number of images")
         H, W = st.geo
-        off = st.lib.mk_workspace_offset(st.h, name.encode(), st.n_img // 2, H, W)
-        if off < 0:
-            raise _lib.MickeyB200Error(st.lib.mk_last_error().decode())
-        n = 1
-        for d in shape:
-            n *= d
-        nbytes = n * torch.empty((), dtype=dtype).element_size()
-        return st.ws[off:off + nbytes].view(dtype).reshape(shape)
+        return st.workspace_view(st.ws, st.n_img // 2, H, W, name, dtype, shape)

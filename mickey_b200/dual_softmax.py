@@ -11,7 +11,6 @@ the backward; no N x N tensor is kept.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 from typing import Optional
 
@@ -23,10 +22,6 @@ from . import _lib
 MAX_N = 8192
 DESC_DIM = 128
 UNIT_NORM_SQ = 1.0005      # squared norms up to this count as unit (|S| <= 1.001, mk_match's bound under NORM_DSC)
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _check_dsc(name, t):
@@ -49,14 +44,6 @@ def _check_scr(name, t, B, N, dev):
         raise ValueError(f"{name} must be float32 on {dev}, got {t.dtype} on {t.device}")
 
 
-def _pitch_view(g, B, N):
-    """(tensor, row pitch): a gradient read in place when its rows are contiguous and pairs lie N row pitches apart."""
-    s0, s1, s2 = g.stride()
-    if s2 == 1 and s1 >= N and (B == 1 or s0 == N * s1):
-        return g, s1
-    return g.contiguous(), N
-
-
 class _DualSoftmax(torch.autograd.Function):
     @staticmethod
     def forward(ctx, dsc0, dsc1, dustbin, scr0, scr1, temperature, unit_norm):
@@ -76,11 +63,11 @@ class _DualSoftmax(torch.autograd.Function):
                 final = torch.empty_like(scores)
             lse_r = torch.empty(B, npad, dtype=torch.float32, device=dev)
             lse_c = torch.empty(B, npad, dtype=torch.float32, device=dev)
-            ws = torch.empty(int(lib.mk_dual_softmax_ws_bytes(B, N)), dtype=torch.uint8, device=dev)
+            ws = _lib.workspace(lib.mk_dual_softmax_ws_bytes(B, N), dev, "mk_dual_softmax_ws_bytes")
             _lib.check(lib.mk_dual_softmax(_lib.ptr(d0), _lib.ptr(d1), _lib.ptr(s0), _lib.ptr(s1), _lib.ptr(db),
                                            float(temperature), B, N, int(unit_norm), _lib.ptr(scores), _lib.ptr(kp),
                                            _lib.ptr(final), N, _lib.ptr(lse_r), _lib.ptr(lse_c), _lib.ptr(ws), ws.numel(),
-                                           _stream(dev)), "mk_dual_softmax")
+                                           _lib.stream(dev)), "mk_dual_softmax")
         ctx.save_for_backward(d0, d1, s0, s1, db, lse_r, lse_c)
         ctx.temperature = float(temperature)
         ctx.scr_shapes = (None if scr0 is None else scr0.shape, None if scr1 is None else scr1.shape)
@@ -99,7 +86,7 @@ class _DualSoftmax(torch.autograd.Function):
         B, _, N = d0.shape
         dev = d0.device
         lib = _lib.load()
-        views = [None if g is None else _pitch_view(g.float(), B, N) for g in (gs, gk, gf)]
+        views = [None if g is None else _lib.pitched(g.float()) for g in (gs, gk, gf)]
         (gs, ps), (gk, pk), (gf, pf) = [(None, 0) if v is None else v for v in views]
         with torch.cuda.device(dev):
             dd0 = torch.empty_like(d0)
@@ -107,12 +94,12 @@ class _DualSoftmax(torch.autograd.Function):
             ds0 = None if s0 is None else torch.empty_like(s0)
             ds1 = None if s1 is None else torch.empty_like(s1)
             ddb = None if db is None else torch.empty(1, dtype=torch.float32, device=dev)
-            ws = torch.empty(int(lib.mk_dual_softmax_backward_ws_bytes(B, N)), dtype=torch.uint8, device=dev)
+            ws = _lib.workspace(lib.mk_dual_softmax_backward_ws_bytes(B, N), dev, "mk_dual_softmax_backward_ws_bytes")
             _lib.check(lib.mk_dual_softmax_backward(
                 _lib.ptr(d0), _lib.ptr(d1), _lib.ptr(s0), _lib.ptr(s1), _lib.ptr(db), ctx.temperature, B, N,
                 _lib.ptr(lse_r), _lib.ptr(lse_c), _lib.ptr(gs), ps, _lib.ptr(gk), pk, _lib.ptr(gf), pf,
                 _lib.ptr(dd0), _lib.ptr(dd1), _lib.ptr(ds0), _lib.ptr(ds1), _lib.ptr(ddb), _lib.ptr(ws), ws.numel(),
-                _stream(dev)), "mk_dual_softmax_backward")
+                _lib.stream(dev)), "mk_dual_softmax_backward")
         sh0, sh1 = ctx.scr_shapes
         return (dd0, dd1,
                 None if ddb is None else ddb.reshape(ctx.dustbin_shape),

@@ -193,6 +193,20 @@ def interpolate_pos_embed(pos_embed: torch.Tensor, gh: int, gw: int) -> torch.Te
     return torch.cat([pe[0, :1], grid.permute(0, 2, 3, 1).reshape(gh * gw, dim)], dim=0)
 
 
+def raw_positions(sd: Dict[str, torch.Tensor], device, prefix: str = BACKBONE):
+    """(pos_embed, cls_token, patch-embedding bias) of a state dict, fp32 on `device`: the inputs of position_tables."""
+    return tuple(sd[prefix + n].detach().to(device).float() for n in ("pos_embed", "cls_token", "patch_embed.proj.bias"))
+
+
+def position_tables(raw, H: int, W: int) -> Dict[str, torch.Tensor]:
+    """The backbone's size-dependent tables for H x W images, from raw_positions(): "patch.posb" (the position embedding
+    resized to the patch grid plus the patch-embedding bias) and "patch.clspos" (the cls token plus its position)."""
+    pos, cls, pbias = raw
+    with torch.no_grad():
+        full = interpolate_pos_embed(pos, H // PATCH, W // PATCH)
+        return {"patch.posb": (full[1:] + pbias[None]).contiguous(), "patch.clspos": (cls.reshape(-1) + full[0]).contiguous()}
+
+
 def sine_table_padded(gh: int, gw: int, d_model: int = 128) -> torch.Tensor:
     """2-D sine position encoding (att_layers/transformer.py:25-36, positions start at 1) laid out on
     the zero-padded token grid: [(gh+2)*(gw+2), d_model], zeros on the pad ring."""
@@ -210,7 +224,7 @@ def sine_table_padded(gh: int, gw: int, d_model: int = 128) -> torch.Tensor:
 
 
 # ---------------------------------------------------------------------------------------------------------
-class Engine:
+class Engine(_lib.Handle):
     """One C handle + packed weights + workspace for a fixed (cfg, device)."""
     MAX_GEOMETRIES = 4          # image geometries whose tables / workspace / graphs are kept alive at once
 
@@ -218,15 +232,12 @@ class Engine:
         """side_stream=True gives the engine its own CUDA stream for forward(): two such engines (see
         MickeyRelativePose.pipeline_depth) keep two steps in flight, so the many kernels of one step that cannot fill
         132 SMs at B=1 share the GPU with the next step's."""
-        self.lib = _lib.load()
         self.cfg = cfg
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
+        device = torch.device(device)
+        if device.type != "cuda":
             raise _lib.MickeyB200Error("mickey_b200 runs on a CUDA device only (sm_90a); there is no CPU path")
         self.mkcfg = make_mk_config(cfg)
-        h = C.c_void_p()
-        _lib.check(self.lib.mk_create(self.device.index or 0, C.byref(self.mkcfg), C.byref(h)), "mk_create")
-        self.h = h
+        super().__init__(device, self.mkcfg)
         self.packed: Dict[str, torch.Tensor] = {}
         self.stream = torch.cuda.Stream(device=self.device) if side_stream else None
         self.assume_inputs_ready = False
@@ -289,13 +300,6 @@ class Engine:
         finally:
             self.stream.wait_stream(caller)
 
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                self.lib.mk_destroy(self.h)
-        except Exception:
-            pass
-
     # -- weights ---------------------------------------------------------------------------------------------
     def load_state_dict(self, sd: Dict[str, torch.Tensor], share_with: "Engine" = None):
         """share_with: another engine on the same device whose packed weight tensors are registered here too
@@ -306,11 +310,9 @@ class Engine:
         else:
             with torch.no_grad():
                 self.packed = pack_weights(sd, self.cfg, self.device)
-                self._raw_pos = (sd[BACKBONE + "pos_embed"].detach().to(self.device).float(),
-                                 sd[BACKBONE + "cls_token"].detach().to(self.device).float(),
-                                 sd[BACKBONE + "patch_embed.proj.bias"].detach().to(self.device).float())
+                self._raw_pos = raw_positions(sd, self.device)
         for name, t in self.packed.items():
-            self._register(name, self._own(t))
+            self.register(name, self._own(t))
         self._caller_pending = True
         # captured graphs hold raw pointers of the previous packed weights and tables: none of them may be replayed
         self._graphs.clear()
@@ -320,17 +322,12 @@ class Engine:
         self.ws = None
         self.ws_pairs = 0
 
-    def _register(self, name, t):
-        assert t.is_contiguous() and t.device == self.device
-        dt = {torch.float32: 0, torch.float16: 1}[t.dtype]
-        _lib.check(self.lib.mk_set_tensor(self.h, name.encode(), _lib.ptr(t), dt, t.numel()), f"mk_set_tensor({name})")
-
     def prepare(self, n_pairs: int, H: int, W: int):
         """Size-dependent tables + workspace for images cropped to (H, W) (multiples of 14)."""
         self._use_geometry(H, W)
         if self.ws is None or self.ws_pairs < n_pairs:
             nbytes = self.lib.mk_workspace_bytes(self.h, n_pairs, H, W)
-            self.ws = self._own(torch.empty(nbytes, dtype=torch.uint8, device=self.device))
+            self.ws = self._own(_lib.workspace(nbytes, self.device, "mk_workspace_bytes"))
             self.ws_pairs = n_pairs
             self._caller_pending = True
         return self.ws
@@ -343,13 +340,8 @@ class Engine:
                 self._geo_state[self.geo].update(ws=self.ws, ws_pairs=self.ws_pairs)
             gs = self._geo_state.get((H, W))
             if gs is None:
-                gh, gw = H // PATCH, W // PATCH
-                with torch.no_grad():
-                    pos, cls, pbias = self._raw_pos
-                    full = interpolate_pos_embed(pos, gh, gw)
-                    gs = {"patch.posb": (full[1:] + pbias[None]).contiguous(),
-                          "patch.clspos": (cls.reshape(-1) + full[0]).contiguous(),
-                          "head.pe": sine_table_padded(gh, gw).to(self.device), "ws": None, "ws_pairs": 0}
+                gs = position_tables(self._raw_pos, H, W)
+                gs.update({"head.pe": sine_table_padded(H // PATCH, W // PATCH).to(self.device), "ws": None, "ws_pairs": 0})
                 for n in ("patch.posb", "patch.clspos", "head.pe"):
                     self._own(gs[n])
                 self._caller_pending = True
@@ -361,7 +353,7 @@ class Engine:
                 self._geo_state[(H, W)] = gs
             for n in ("patch.posb", "patch.clspos", "head.pe"):
                 self.packed[n] = gs[n]
-                self._register(n, gs[n])
+                self.register(n, gs[n])
             _lib.check(self.lib.mk_finalize(self.h, H, W), "mk_finalize")
             self.geo = (H, W)
             self.ws, self.ws_pairs = gs["ws"], gs["ws_pairs"]
@@ -379,14 +371,7 @@ class Engine:
     def ws_view(self, name: str, dtype, shape):
         """Typed view of a named intermediate buffer of the last call's workspace (debugging / tests)."""
         H, W = self.geo
-        off = self.lib.mk_workspace_offset(self.h, name.encode(), self.ws_pairs, H, W)
-        if off < 0:
-            raise _lib.MickeyB200Error(self.lib.mk_last_error().decode())
-        n = 1
-        for d in shape:
-            n *= d
-        nbytes = n * torch.empty((), dtype=dtype).element_size()
-        return self.ws[off:off + nbytes].view(dtype).reshape(shape)
+        return self.workspace_view(self.ws, self.ws_pairs, H, W, name, dtype, shape)
 
     def profile(self, enable: bool):
         _lib.check(self.lib.mk_profile_enable(self.h, int(enable)), "mk_profile_enable")
@@ -407,14 +392,10 @@ class Engine:
         if self.ws_pairs != n_pairs:
             nbytes = self.lib.mk_workspace_bytes(self.h, n_pairs, H, W)
             if self.ws.numel() < nbytes:
-                self.ws = self._own(torch.empty(nbytes, dtype=torch.uint8, device=self.device))
+                self.ws = self._own(_lib.workspace(nbytes, self.device, "mk_workspace_bytes"))
                 self._caller_pending = True
             self.ws_pairs = n_pairs
         return self.ws
-
-    @staticmethod
-    def _stream():
-        return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
     # -- stages ------------------------------------------------------------------------------------------------
     @staticmethod
@@ -447,7 +428,7 @@ class Engine:
         fn = self.lib.mk_extract_u8 if u8 else self.lib.mk_extract
         with self._ordered():
             _lib.check(fn(self.h, _lib.ptr(images), B, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
-                          _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), self._stream()), "mk_extract")
+                          _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), _lib.stream()), "mk_extract")
         return kps, depth, scr, dsc
 
     # -- feature banks: extract images once, then match / solve any pairs among them ------------------------------
@@ -457,7 +438,7 @@ class Engine:
         nbytes = self.lib.mk_workspace_bytes_for(self.h, n_img, n_pairs, H, W)
         if self._pairs_ws is None or self._pairs_ws.numel() < nbytes:
             self._pairs_ws = None
-            self._pairs_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            self._pairs_ws = _lib.workspace(nbytes, self.device, "mk_workspace_bytes_for")
         return self._pairs_ws
 
     def extract_images(self, images: torch.Tensor):
@@ -473,7 +454,7 @@ class Engine:
         fn = self.lib.mk_extract_images_u8 if u8 else self.lib.mk_extract_images
         with self._ordered():
             _lib.check(fn(self.h, _lib.ptr(images), n_img, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
-                          _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), self._stream()), "mk_extract_images")
+                          _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), _lib.stream()), "mk_extract_images")
         return kps, depth, scr, dsc
 
     def forward_pairs(self, bank0, idx0, bank1, idx1, K0, K1, seed: int, image_size, lean: bool = False):
@@ -503,7 +484,7 @@ class Engine:
                 self.h, *(p(t) for t in bank0), bank0[0].shape[0], *(p(t) for t in bank1), bank1[0].shape[0], p(idx0), p(idx1),
                 p(K0), p(K1), P, C.c_ulonglong(seed), p(out["kps"]), p(out["depth"]), p(out["scores"]), p(out["kp_scores"]),
                 p(out["final_scores"]), out["final_scores"].stride(1), p(out["pose"]), p(out["best_set"]), p(out["inlier_mask"]),
-                p(out["sampled_idx"]), p(out["status"]), p(ws), ws.numel(), self._stream()), "mk_forward_pairs")
+                p(out["sampled_idx"]), p(out["status"]), p(ws), ws.numel(), _lib.stream()), "mk_forward_pairs")
         return out
 
     def match(self, B: int, N: int, lean: bool = False):
@@ -514,7 +495,7 @@ class Engine:
         final = nn_empty(B, N, dev)
         with self._ordered():
             _lib.check(self.lib.mk_match(self.h, B, _lib.ptr(scores), _lib.ptr(kp_scores), _lib.ptr(final), final.stride(1),
-                                         _lib.ptr(self.ws), self.ws.numel(), self._stream()), "mk_match")
+                                         _lib.ptr(self.ws), self.ws.numel(), _lib.stream()), "mk_match")
         return scores, kp_scores, final
 
     # -- whole path in one C call, optionally replayed from a CUDA graph -------------------------------------------
@@ -541,7 +522,7 @@ class Engine:
             _lib.ptr(st["kps"]), _lib.ptr(st["depth"]), _lib.ptr(st["scr"]), _lib.ptr(st["dsc"]), _lib.ptr(st["scores"]),
             _lib.ptr(st["kp_scores"]), _lib.ptr(st["final_scores"]), st["final_scores"].stride(1), _lib.ptr(st["pose"]), _lib.ptr(st["best_set"]),
             _lib.ptr(st["inlier_mask"]), _lib.ptr(st["sampled_idx"]), _lib.ptr(st["status"]), _lib.ptr(ws), ws.numel(),
-            self._stream()), "mk_forward")
+            _lib.stream()), "mk_forward")
 
     def forward(self, image0, image1, K0, K1, seed: int, use_graph: bool = True, lean: bool = False):
         """Whole hot path (extract -> match -> solve) for a batch of pairs.
@@ -641,7 +622,7 @@ class Engine:
             ent["launches"] = self.launch_count - l0
             ent["calls"] = 1
         else:
-            _lib.check(self.lib.mk_set_seed(self.h, C.c_ulonglong(seed), self._stream()), "mk_set_seed")
+            _lib.check(self.lib.mk_set_seed(self.h, C.c_ulonglong(seed), _lib.stream()), "mk_set_seed")
             if ent["graph"] is None:
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
@@ -658,8 +639,7 @@ class Engine:
         """kps [2B,2,N], depth [2B,1,N] as produced by extract (image0 rows first).  final_scores [B,N,N] may be a padded
         view (last dim contiguous, rows `stride(1)` floats apart) or any tensor (made contiguous)."""
         B, N, _ = final_scores.shape
-        if final_scores.stride(2) != 1 or final_scores.stride(0) != N * final_scores.stride(1):
-            final_scores = final_scores.contiguous()
+        final_scores, pitch = _lib.pitched(final_scores)
         dev = self.device
         c = self.mkcfg
         pose = torch.empty(B, 13, device=dev)
@@ -676,9 +656,9 @@ class Engine:
         K1 = K1.to(dev, torch.float32).contiguous()
         with self._ordered():
             _lib.check(self.lib.mk_solve_pose(
-                self.h, _lib.ptr(final_scores), final_scores.stride(1), _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(K0), _lib.ptr(K1), B, N,
+                self.h, _lib.ptr(final_scores), pitch, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(K0), _lib.ptr(K1), B, N,
                 C.c_ulonglong(seed & (2 ** 64 - 1)), _lib.ptr(outer_idx), _lib.ptr(inner_idx), _lib.ptr(pose),
                 _lib.ptr(best_set), _lib.ptr(mask), _lib.ptr(sampled), _lib.ptr(hyp), _lib.ptr(status),
-                _lib.ptr(self.ws), self.ws.numel(), self._stream()), "mk_solve_pose")
+                _lib.ptr(self.ws), self.ws.numel(), _lib.stream()), "mk_solve_pose")
         return {"pose": pose, "status": status, "best_set": best_set, "inlier_mask": mask, "sampled_idx": sampled,
                 "hyp_scores": hyp}

@@ -11,7 +11,6 @@ INTEGRATION.md shows the swap in a training model.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 
 import torch
@@ -27,10 +26,6 @@ MAX_B = 65535                 # the kernels' per-image grids (gridDim.y)
 MAX_TOKENS = 65535 * 64       # the GEMMs' 64-token tiles (gridDim.y)
 MAX_LAYERS = 1024
 _NAMES = ("q_proj", "k_proj", "v_proj", "merge", "mlp0", "mlp2", "norm1_w", "norm1_b", "norm2_w", "norm2_b")
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _layer_table(params, num_layers):
@@ -54,9 +49,10 @@ def _forward(x, pe, params, num_layers, save):
     lib = _lib.load()
     with torch.cuda.device(dev):
         out = torch.empty(B, D_MODEL, h, w, dtype=torch.float32, device=dev)
-        ws = torch.empty(int(lib.mk_head_transformer_ws_bytes(B, h, w, num_layers, int(save))), dtype=torch.uint8, device=dev)
+        ws = _lib.workspace(lib.mk_head_transformer_ws_bytes(B, h, w, num_layers, int(save)), dev,
+                            "mk_head_transformer_ws_bytes")
         _lib.check(lib.mk_head_transformer(_lib.ptr(x), _lib.ptr(pe), B, h, w, _layer_table(params, num_layers), num_layers,
-                                           _lib.ptr(out), int(save), _lib.ptr(ws), ws.numel(), _stream(dev)),
+                                           _lib.ptr(out), int(save), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                    "mk_head_transformer")
     return out, ws
 
@@ -89,9 +85,10 @@ class _HeadTransformer(torch.autograd.Function):
                 for j, name in enumerate(_NAMES):
                     t = grads[10 * i + j]
                     setattr(gtab[i], name, None if t is None else t.data_ptr())
-            ws = torch.empty(int(lib.mk_head_transformer_backward_ws_bytes(B, h, w, L)), dtype=torch.uint8, device=dev)
+            ws = _lib.workspace(lib.mk_head_transformer_backward_ws_bytes(B, h, w, L), dev,
+                                "mk_head_transformer_backward_ws_bytes")
             _lib.check(lib.mk_head_transformer_backward(_lib.ptr(saved), _lib.ptr(g), B, h, w, _layer_table(params, L), L,
-                                                        _lib.ptr(gx), gtab, _lib.ptr(ws), ws.numel(), _stream(dev)),
+                                                        _lib.ptr(gx), gtab, _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                        "mk_head_transformer_backward")
         return (gx, None, None, *grads)
 

@@ -19,8 +19,6 @@ Edge behaviour follows the reference:
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 import torch
 
@@ -29,10 +27,6 @@ from . import _lib
 STATUS_PRECHECK, STATUS_INNER = 16, 32          # include/mickey_b200.h MK_LOSS_STATUS_*
 STATUS_SKIP = 1 | 2 | STATUS_PRECHECK | STATUS_INNER
 LOSS_MAX_S, LOSS_MAX_C = 2048, 16              # csrc/ops.h: largest NUM_SAMPLES_MATCHES and NUM_CORR_3d3d
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def vcre_grid(device=None) -> torch.Tensor:
@@ -162,10 +156,7 @@ def loss_search(fs, kps0, d0, kps1, d1, K0, K1, p: LossParams, seed: int, outer_
     [B*IM*IR, S], status int).  final_scores may be a view with contiguous rows and pairs N row pitches apart."""
     B, N = fs.shape[0], fs.shape[1]
     IM, IR, S, Cn = p.it_matches, p.it_ransac, p.n_sample, p.num_corr
-    s0, s1, s2 = fs.stride()
-    if not (s2 == 1 and s1 >= N and (B == 1 or s0 == N * s1)):
-        fs = fs.contiguous()
-        s1 = N
+    fs, pitch = _lib.pitched(fs)
     dev = fs.device
     f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
     kps0, d0, kps1, d1, K0, K1 = (f32(t) for t in (kps0, d0, kps1, d1, K0, K1))
@@ -174,18 +165,17 @@ def loss_search(fs, kps0, d0, kps1, d1, K0, K1, p: LossParams, seed: int, outer_
     inner = torch.empty(B * IM * IR, Cn, dtype=torch.int32, device=dev)
     bits = torch.empty(B * IM * IR, S // 32, dtype=torch.int32, device=dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
-    ws_bytes = int(lib.mk_loss_search_ws_bytes(B, IM))
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    ws = _lib.workspace(lib.mk_loss_search_ws_bytes(B, IM), dev, "mk_loss_search_ws_bytes")
     oi = None if outer_idx is None else outer_idx.to(dev, torch.int32).contiguous()
     ii = None if inner_idx is None else inner_idx.to(dev, torch.int32).contiguous()
     if oi is not None and tuple(oi.shape) != (B * IM, S):
         raise ValueError(f"outer_idx must be [B*IM, S] = [{B * IM}, {S}], got {tuple(oi.shape)}")
     if ii is not None and tuple(ii.shape) != (B * IM * IR, Cn):
         raise ValueError(f"inner_idx must be [B*IM*IR, C] = [{B * IM * IR}, {Cn}], got {tuple(ii.shape)}")
-    _lib.check(lib.mk_loss_search(_lib.ptr(fs), s1, _lib.ptr(kps0), _lib.ptr(d0), _lib.ptr(kps1), _lib.ptr(d1), _lib.ptr(K0),
+    _lib.check(lib.mk_loss_search(_lib.ptr(fs), pitch, _lib.ptr(kps0), _lib.ptr(d0), _lib.ptr(kps1), _lib.ptr(d1), _lib.ptr(K0),
                                   _lib.ptr(K1), B, N, IM, IR, S, Cn, p.num_ref_steps, p.inlier_ref_th, seed, _lib.ptr(oi),
                                   _lib.ptr(ii), _lib.ptr(sampled), _lib.ptr(inner), _lib.ptr(bits), _lib.ptr(status),
-                                  _lib.ptr(ws), ws_bytes, _stream(dev)), "mk_loss_search")
+                                  _lib.ptr(ws), ws.numel(), _lib.stream(dev)), "mk_loss_search")
     return sampled, inner, unpack_mask(bits, S), int(status.item())
 
 
@@ -196,10 +186,9 @@ def loss_gradient(sampled, loss_value, baseline, mask_topk, B, N, IM, S):
     f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
     lv, bl, mk = f32(loss_value).reshape(-1), f32(baseline).reshape(-1), f32(mask_topk).reshape(-1)
     grad = torch.empty(B, N, N, dtype=torch.float32, device=dev)
-    ws_bytes = int(lib.mk_loss_gradient_ws_bytes(B, IM, S))
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    ws = _lib.workspace(lib.mk_loss_gradient_ws_bytes(B, IM, S), dev, "mk_loss_gradient_ws_bytes")
     _lib.check(lib.mk_loss_gradient(_lib.ptr(sampled.to(torch.int32).contiguous()), _lib.ptr(lv), _lib.ptr(bl), _lib.ptr(mk),
-                                    B, N, IM, S, _lib.ptr(grad), _lib.ptr(ws), ws_bytes, _stream(dev)), "mk_loss_gradient")
+                                    B, N, IM, S, _lib.ptr(grad), _lib.ptr(ws), ws.numel(), _lib.stream(dev)), "mk_loss_gradient")
     return grad
 
 

@@ -7,7 +7,6 @@ zero rows make them common) are ordered by ascending i, which the reference's un
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 from typing import List, Tuple
 
@@ -52,10 +51,7 @@ def mutual_matches_raw(scores: torch.Tensor, min_conf: float = 0.0):
     min_conf = _check_min_conf(min_conf)
     scores = _check_scores(scores)
     B, N = scores.shape[0], scores.shape[1]
-    s0, s1, s2 = scores.stride()
-    if not (s2 == 1 and s1 >= N and (B == 1 or s0 == N * s1)):
-        scores = scores.contiguous()
-        s1 = N
+    scores, pitch = _lib.pitched(scores)
     lib = _lib.load()
     dev = scores.device
     W = N - 1
@@ -63,10 +59,9 @@ def mutual_matches_raw(scores: torch.Tensor, min_conf: float = 0.0):
         matches = torch.empty(B, W, 2, dtype=torch.int32, device=dev)
         match_scores = torch.empty(B, W, dtype=torch.float32, device=dev)
         count = torch.empty(B, dtype=torch.int32, device=dev)
-        ws = torch.empty(int(lib.mk_mutual_matches_ws_bytes(B, N)), dtype=torch.uint8, device=dev)
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(lib.mk_mutual_matches(_lib.ptr(scores), s1, B, N, min_conf, _lib.ptr(matches), _lib.ptr(match_scores),
-                                         _lib.ptr(count), _lib.ptr(ws), ws.numel(), stream), "mk_mutual_matches")
+        ws = _lib.workspace(lib.mk_mutual_matches_ws_bytes(B, N), dev, "mk_mutual_matches_ws_bytes")
+        _lib.check(lib.mk_mutual_matches(_lib.ptr(scores), pitch, B, N, min_conf, _lib.ptr(matches), _lib.ptr(match_scores),
+                                         _lib.ptr(count), _lib.ptr(ws), ws.numel(), _lib.stream(dev)), "mk_mutual_matches")
     return matches, match_scores, count
 
 

@@ -28,10 +28,6 @@ MAX_CHANNELS = 4096
 TRAIN, RELU, SAVE, BN = 1, 2, 4, 8
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def _strides(t):
     return (C.c_longlong * 4)(*t.stride())
 
@@ -54,11 +50,11 @@ def _forward(x, w1, w2, wsc, bn1, bn2, mom1, mom2, flags):
     lib = _lib.load()
     with torch.cuda.device(dev):
         out = torch.empty(B, cout, h, w, dtype=torch.float32, device=dev)
-        saved = torch.empty(int(lib.mk_resblock_saved_bytes(B, h, w, cin, cout)), dtype=torch.uint8, device=dev)
-        ws = torch.empty(int(lib.mk_resblock_ws_bytes(B, h, w, cin, cout)), dtype=torch.uint8, device=dev)
+        saved = _lib.workspace(lib.mk_resblock_saved_bytes(B, h, w, cin, cout), dev, "mk_resblock_saved_bytes")
+        ws = _lib.workspace(lib.mk_resblock_ws_bytes(B, h, w, cin, cout), dev, "mk_resblock_ws_bytes")
         P = _params(w1, w2, wsc, bn1, bn2, mom1, mom2)
         _lib.check(lib.mk_resblock_forward(_lib.ptr(x), _strides(x), B, h, w, cin, cout, C.byref(P), flags, _lib.ptr(out),
-                                           _lib.ptr(saved), saved.numel(), _lib.ptr(ws), ws.numel(), _stream(dev)),
+                                           _lib.ptr(saved), saved.numel(), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
                    "mk_resblock_forward")
     return out, saved       # the scratch workspace is released here; only the saved region outlives the call
 
@@ -100,10 +96,10 @@ class _ResBlock(torch.autograd.Function):
             P.w1, P.w2, P.wsc = w1.data_ptr(), w2.data_ptr(), None if wsc is None else wsc.data_ptr()
             if g1 is not None:
                 P.bn1_w, P.bn2_w = g1.data_ptr(), g2.data_ptr()
-            ws = torch.empty(int(lib.mk_resblock_backward_ws_bytes(B, h, w, cin, cout)), dtype=torch.uint8, device=dev)
+            ws = _lib.workspace(lib.mk_resblock_backward_ws_bytes(B, h, w, cin, cout), dev, "mk_resblock_backward_ws_bytes")
             _lib.check(lib.mk_resblock_backward(_lib.ptr(saved), _lib.ptr(g), _strides(g), _lib.ptr(out), B, h, w, cin, cout,
                                                 C.byref(P), ctx.flags, want, C.byref(G), _lib.ptr(ws), ws.numel(),
-                                                _stream(dev)),
+                                                _lib.stream(dev)),
                        "mk_resblock_backward")
         return (*grads, None, None, None, None, None)
 

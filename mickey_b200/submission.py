@@ -11,7 +11,6 @@ differs in the 7th digit).
 """
 from __future__ import annotations
 
-import ctypes as C
 from collections import defaultdict
 from dataclasses import dataclass
 from pathlib import Path
@@ -53,8 +52,7 @@ def poses_to_records(packed: torch.Tensor) -> np.ndarray:
     B = packed.shape[0]
     out = torch.empty(B, 9, dtype=torch.float64, device=packed.device)
     with torch.cuda.device(packed.device):
-        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        _lib.check(lib.mk_pose_to_submission(_lib.ptr(packed), B, _lib.ptr(out), stream), "mk_pose_to_submission")
+        _lib.check(lib.mk_pose_to_submission(_lib.ptr(packed), B, _lib.ptr(out), _lib.stream()), "mk_pose_to_submission")
     return out.cpu().numpy()
 
 

@@ -116,8 +116,8 @@ def test_abi_library_loads_and_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), name
     assert b"sm_90a" in lib.mk_version()
-    assert ctypes.sizeof(_lib.MkConfig) == lib.mk_sizeof_config()
-    assert ctypes.sizeof(_lib.MkGemmArgs) == lib.mk_sizeof_gemm_args()
+    assert ctypes.sizeof(_lib.MkConfig) == lib.mk_sizeof(b"mk_config")
+    assert ctypes.sizeof(_lib.MkGemmArgs) == lib.mk_sizeof(b"mk_gemm_args")
 
 
 def test_hot_kernels_are_tcgen05_tma_tmem_in_sass():
