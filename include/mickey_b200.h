@@ -362,6 +362,46 @@ int mk_resblock_backward(const void* saved_dev, const float* grad_out_dev, const
                          int flags, int want, const mk_resblock_grads* grads_host, void* ws_dev, long long ws_bytes,
                          void* stream);
 
+/* ---- training: the heads' output layers (mickey_extractor.py:81-142, 160-178, 199-218, 246-249), forward and backward
+ * in fp32 (mickey_b200/heads.py wraps both as a torch.autograd.Function).  No handle.  x = rb4's output.
+ *
+ * kind                  weight   output [B, k, h, w]
+ * MK_HO_SCORE_SOFTMAX   [1, C]   p = e / (sum e + eps), e = exp((r - (mean r + eps)) / temperature) mask, per image
+ * MK_HO_SCORE_SIGMOID   [1, C]   sigmoid(r) mask
+ * MK_HO_OFFSET          [2, C]   sigmoid(r)
+ * MK_HO_DEPTH           [1, C]   r
+ * MK_HO_DEPTH_SIGMOID   [1, C]   max_depth sigmoid(r)
+ * MK_HO_DESC_L2         NULL     x / sqrt(sum_c x^2 + 1e-10)                                  (k = C)
+ * with r = W x (the 1x1 convolution) and mask zeroing 3 cells at each border.  eps_dev is a device scalar (the det head's
+ * `eps` Parameter), read by the kernel.
+ *
+ * mk_head_out_forward: x_dev fp32 [B, C, h, w] with element strides x_strides_host[4] (any layout); weight_dev fp32 [k, C]
+ * contiguous; out_dev fp32 [B, k, h, w] contiguous.  norm_dev fp32 [B, h, w] receives the descriptor's per-pixel norm for
+ * the backward (MK_HO_DESC_L2 only; NULL skips it).
+ * mk_head_out_backward: out_dev and norm_dev as the forward wrote them, grad_out_dev fp32 [B, k, h, w] contiguous; grad_x_dev
+ * fp32 [B, C, h, w] contiguous and grad_w_dev fp32 [k, C] (no weight gradient for MK_HO_DESC_L2), each NULL to skip, and
+ * overwritten, not accumulated.  x_dev is read only for the weight gradient.  Workspace: mk_head_out_backward_ws_bytes
+ * bytes, 256-byte aligned (0 for MK_HO_DESC_L2; -1 for a bad geometry).
+ *
+ * All arithmetic is fp32; the per-image and per-pixel reductions and the weight gradient's pixel slots accumulate in fp64 in
+ * a fixed order.  No atomics: bit-identical run to run, an image's output and input gradient do not depend on the rest of
+ * the batch, and every layout of x gives the same bits.  Limits: B, h, w >= 1, B h w <= 2^26, 1 <= C <= 4096.  Bad
+ * arguments return MK_ERR_INVALID and launch nothing. */
+#define MK_HO_SCORE_SOFTMAX 0
+#define MK_HO_SCORE_SIGMOID 1
+#define MK_HO_OFFSET 2
+#define MK_HO_DEPTH 3
+#define MK_HO_DEPTH_SIGMOID 4
+#define MK_HO_DESC_L2 5
+long long mk_head_out_backward_ws_bytes(int kind, int B, int h, int w, int C);
+int mk_head_out_forward(int kind, const float* x_dev, const long long* x_strides_host, int B, int C, int h, int w,
+                        const float* weight_dev, const float* eps_dev, float temperature, float max_depth, float* out_dev,
+                        float* norm_dev, void* stream);
+int mk_head_out_backward(int kind, const float* x_dev, const long long* x_strides_host, int B, int C, int h, int w,
+                         const float* weight_dev, float temperature, float max_depth, const float* out_dev,
+                         const float* norm_dev, const float* grad_out_dev, float* grad_x_dev, float* grad_w_dev, void* ws_dev,
+                         long long ws_bytes, void* stream);
+
 /* (Re)seed the solver's device-side generator on `stream` (used in front of a CUDA-graph replay of mk_forward
  * captured with seed = 0). */
 int mk_set_seed(mk_handle* h, unsigned long long seed, void* stream);

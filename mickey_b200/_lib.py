@@ -156,6 +156,12 @@ EXPORTS = {
     "mk_resblock_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong), C.c_void_p, C.c_int, C.c_int,
                                        C.c_int, C.c_int, C.c_int, C.POINTER(MkResblockParams), C.c_int, C.c_int,
                                        C.POINTER(MkResblockGrads), C.c_void_p, C.c_longlong, C.c_void_p]),
+    "mk_head_out_backward_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_head_out_forward": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mk_head_out_backward": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(C.c_longlong), C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
     "mk_pose_to_submission": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "mk_launch_count": (C.c_longlong, [C.c_void_p]),
     "mk_pdl_enabled": (C.c_int, []),
