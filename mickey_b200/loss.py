@@ -208,7 +208,10 @@ class MetricPoseLoss(torch.nn.Module):
 
     def _vcre_grid(self, dev):
         if dev not in self._grid:
-            self._grid[dev] = vcre_grid(dev).float()
+            # a normal tensor even when the first call is a validation under inference mode (Lightning's default, and its
+            # sanity check runs before the first training step): autograd cannot save an inference tensor for backward
+            with torch.inference_mode(False):
+                self._grid[dev] = vcre_grid(dev).float()
         return self._grid[dev]
 
     def forward(self, batch, seed=None, outer_idx=None, inner_idx=None):

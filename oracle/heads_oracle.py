@@ -1,4 +1,4 @@
-"""Plain-torch restatement of the heads' output layers with a closed-form backward, and of a whole head in train mode.
+"""Plain-torch restatement of the heads' output layers with a closed-form backward, and of a whole head in train or eval mode.
 
 Output layers (x = rb4's output [B, C, h, w], W the 1x1 weight [k, C], r = W x, g the upstream gradient):
     score_softmax   remove_brd_and_softmax (mickey_extractor.py:98-124, 137-138): s = r - (mean r + eps) with the mean
@@ -9,7 +9,7 @@ Output layers (x = rb4's output [B, C, h, w], W the 1x1 weight [k, C], r = W x, 
     desc            desc_l2norm (extractor_utils.py:6-10), y = x / n;        dx = (g - y (y . g)) / n
 and for the convolution dx = dr^T W, dW = sum_{b, p} dr x^T.  mask zeroes 3 cells at each border.
 
-head_chain restates a head's forward in train mode: resblock1..3 (oracle/resblock_oracle.py), the transformer
+head_chain restates a head's forward in train or eval mode: resblock1..3 (oracle/resblock_oracle.py), the transformer
 (oracle/mickey_oracle.py head_transformer), resblock4 (relu=False for the descriptor head, :246) and the output layer, as
 mickey_extractor.py:126-142 / 164-178 / 203-218 / 240-251 chain them.  Device- and dtype-agnostic: everything computes in
 the dtype of its inputs.
@@ -97,10 +97,11 @@ def head_kind(head_name, config):
     return ("desc" if config["DSC_HEAD"]["NORM_DSC"] else None), None, False
 
 
-def head_chain(sd, head_name, config, x, momentum=0.1):
-    """A head's train-mode forward on feature_volume x from its state dict `sd` (tensors in the dtype and on the device to
-    compute in; parameters may require grad).  Returns (out, running): running maps every BN running-statistics name to
-    its value after the call, as F.batch_norm leaves it."""
+def head_chain(sd, head_name, config, x, momentum=0.1, train=True):
+    """A head's forward on feature_volume x from its state dict `sd` (tensors in the dtype and on the device to compute
+    in; parameters may require grad).  Returns (out, running): in train mode running maps every BN running-statistics name
+    to its value after the call, as F.batch_norm leaves it; with train=False batch norm uses the running statistics,
+    nothing is updated and running is empty."""
     kind, wname, last_relu = head_kind(head_name, config)
     running = {}
     bn = config["KP_HEADS"]["BN"]
@@ -116,10 +117,10 @@ def head_chain(sd, head_name, config, x, momentum=0.1):
             bns.append(dict(weight=sd[b + "weight"], bias=sd[b + "bias"], running_mean=sd[b + "running_mean"],
                             running_var=sd[b + "running_var"], eps=1e-5, factor=momentum if momentum else 1.0 / nbt))
         wsc = sd.get(pre + "shortcut.0.weight")
-        x, aux = rbo.block_forward(x, sd[pre + "conv1.weight"], sd[pre + "conv2.weight"], wsc, bns[0], bns[1], train=True,
+        x, aux = rbo.block_forward(x, sd[pre + "conv1.weight"], sd[pre + "conv2.weight"], wsc, bns[0], bns[1], train=train,
                                    relu=last_relu or k < 4)
         for j, p in ((1, bns[0]), (2, bns[1])):
-            if p is not None:
+            if p is not None and train:
                 m, v = aux[f"mean{j}"].detach(), aux[f"var{j}"].detach()
                 count = x.numel() // x.shape[1]
                 rm, rv = rbo.running_update(p, m, v, count)

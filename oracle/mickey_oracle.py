@@ -220,9 +220,11 @@ def extractor(sd, img: Tensor, cfg) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
     B, _, H, W = img.shape
     img = img[:, :, : f * (H // f), : f * (W // f)]
     # FLOAT16: True (mickey_extractor.py:31-35,49) == backbone weights stored in fp16: the image is cast to the
-    # backbone's dtype and the patch tokens come back as fp32 (used by bench.py's eager-CUDA comparator)
+    # backbone's dtype and the patch tokens come back as fp32 (used by bench.py's eager-CUDA comparator), or as fp64
+    # when the heads' weights are fp64
     wdt = sd[BACKBONE + "patch_embed.proj.weight"].dtype
-    tok = vit_forward_features(sd, img.to(wdt)).float()
+    hdt = torch.float64 if sd[EXTRACTOR + "det_head.resblock1.conv1.weight"].dtype == torch.float64 else torch.float32
+    tok = vit_forward_features(sd, img.to(wdt)).to(hdt)
     feat = tok.permute(0, 2, 1).reshape(B, -1, H // f, W // f)
     kp, ds = m["KP_HEADS"], m["DSC_HEAD"]
     bn = kp["BN"]
