@@ -420,7 +420,8 @@ int mk_profile_read(mk_handle* h, char* buf, int buf_bytes);
 typedef struct mk_gemm_args {
   int epi;                 /* 0 STORE_H, 1 RESID_F, 2 PATCH, 3 CONV, 4 STORE_F, 5 LN, 6 LSE (row + column partials), 7 DUAL,
                               8 RESID_LN (RESID_F, then out_h = LayerNorm(out_f row) * aux + beta; N <= 1024) */
-  int impl;                /* 0 default (wgmma), 1 wgmma, 2 SIMT debug kernel */
+  int impl;                /* 0 default (wgmma), 1 wgmma, 2 SIMT debug kernel; 3 / 4: the persistent wgmma kernel with /
+                              without two-CTA pairs sharing B, on any grid (the epilogues it does not serve run as 1) */
   const void* a; long long a_rows, a_cols, a_ld;
   const void* b; long long b_rows, b_cols, b_ld;
   int M, N, k_chunks, chunks_per_tap, num_taps;

@@ -173,10 +173,22 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, int g, int m
 }
 
 // ---- staged (coalesced) epilogue -----------------------------------------------------------------------
-// The wgmma kernel first parks a warp's 32 x W block of fp32 accumulators in shared memory (row-major,
-// leading dimension W + 4) and then calls epilogue_rows: lane l owns columns col_base + l*CPL .. (CPL = W/32) of
+// The wgmma kernel first parks a warp's 32 x W block of fp32 accumulators in shared memory (rows of W floats, the
+// 16-byte chunks of a row XOR-swizzled by acc_idx) and then calls epilogue_rows: lane l owns columns col_base + l*CPL .. (CPL = W/32) of
 // every row, so each global load/store instruction of the warp covers ONE contiguous row segment (128-256 B)
 // instead of 32 different rows — 4-8x fewer L1 wavefronts than the thread-per-row form above.
+// Float offset of element (r, c) of a staged 32 x W block (W = 32 or 64).  Chunk k = c / 4 of row r is stored at chunk
+// k ^ h with h = 2 (r % 4) + ((r ^ r / 4 ^ k / 8) & 1) < 8, a permutation of the row's chunks that keeps 16-byte
+// accesses whole.  Every access pattern of the block is free of bank conflicts: the park's float2 stores (rows r..r+3,
+// chunks 2m, 2m + 1 per half-warp), acc_chunk's float4 reads (one chunk of rows 0..7 per quarter-warp), epilogue_rows'
+// float4 reads (chunks 0, 2, .., 14 of one row, or 0, 2, 4, 6 of rows 2t, 2t + 1) and the float2 rows of EPI_RESID_LN.
+// A row stride of W + 4 left the park's stores 2-way conflicted while the tensor cores wait for it.
+template <int W> __device__ __forceinline__ int acc_idx(int r, int c) {
+  const int k = c >> 2;
+  const int h = 2 * (r & 3) + ((r ^ (r >> 2) ^ (k >> 3)) & 1);
+  return r * W + ((k ^ h) << 2) + (c & 3);
+}
+
 template <int CPL> struct VecF;
 template <> struct VecF<1> { using T = float; };
 template <> struct VecF<2> { using T = float2; };
@@ -219,7 +231,7 @@ __device__ __forceinline__ float warp_rowsum32(float (&part)[32], int lane) {
 // pass 1: x = out_f + gamma * (acc + bias) -> out_f (fp32, in place) and back into the staging block; returns the
 // sum of row (lane) over the warp's 64 columns.  Rows at or beyond p.M contribute zeros and are not stored.
 __device__ __forceinline__ float resid_ln_pass1(const GemmParams& p, int row0, int lane, int col_base, float* stage) {
-  constexpr int LDS = 64 + 4, RB = 8;
+  constexpr int RB = 8;
   const int col = col_base + lane * 2;
   const float2 bias = __ldg(reinterpret_cast<const float2*>(p.bias + col)), gam = __ldg(reinterpret_cast<const float2*>(p.gamma + col));
   const int rows = min(32, p.M - row0);
@@ -230,7 +242,7 @@ __device__ __forceinline__ float resid_ln_pass1(const GemmParams& p, int row0, i
 #pragma unroll
     for (int i = 0; i < RB; ++i) {
       const int r = r0 + i;
-      v[i] = *reinterpret_cast<const float2*>(stage + r * LDS + lane * 2);
+      v[i] = *reinterpret_cast<const float2*>(stage + acc_idx<64>(r, lane * 2));
       x[i] = make_float2(0.f, 0.f);
       if (r < rows) x[i] = *reinterpret_cast<const float2*>(p.out_f + (size_t)(row0 + r) * p.out_f_ld + col);
     }
@@ -242,7 +254,7 @@ __device__ __forceinline__ float resid_ln_pass1(const GemmParams& p, int row0, i
         y.x = fmaf(gam.x, v[i].x + bias.x, x[i].x); y.y = fmaf(gam.y, v[i].y + bias.y, x[i].y);
         *reinterpret_cast<float2*>(p.out_f + (size_t)(row0 + r) * p.out_f_ld + col) = y;
       }
-      *reinterpret_cast<float2*>(stage + r * LDS + lane * 2) = y;
+      *reinterpret_cast<float2*>(stage + acc_idx<64>(r, lane * 2)) = y;
       part[r] = y.x + y.y;
     }
   }
@@ -251,11 +263,10 @@ __device__ __forceinline__ float resid_ln_pass1(const GemmParams& p, int row0, i
 
 // pass 2: sum over the warp's 64 columns of (x - mean_row)^2; mean_l holds the mean of row (lane)
 __device__ __forceinline__ float resid_ln_pass2(int lane, const float* stage, float mean_l) {
-  constexpr int LDS = 64 + 4;
   float part[32];
 #pragma unroll
   for (int r = 0; r < 32; ++r) {
-    const float2 x = *reinterpret_cast<const float2*>(stage + r * LDS + lane * 2);
+    const float2 x = *reinterpret_cast<const float2*>(stage + acc_idx<64>(r, lane * 2));
     const float mean = __shfl_sync(0xffffffffu, mean_l, r);
     const float d0 = x.x - mean, d1 = x.y - mean;
     part[r] = d0 * d0 + d1 * d1;
@@ -266,13 +277,12 @@ __device__ __forceinline__ float resid_ln_pass2(int lane, const float* stage, fl
 // pass 3: out_h = (x - mean) * rstd * ln_w + ln_b   (ln_w = p.aux, ln_b = p.beta)
 __device__ __forceinline__ void resid_ln_pass3(const GemmParams& p, int row0, int lane, int col_base, const float* stage,
                                                float mean_l, float rstd_l) {
-  constexpr int LDS = 64 + 4;
   const int col = col_base + lane * 2;
   const float2 w = __ldg(reinterpret_cast<const float2*>(p.aux + col)), b = __ldg(reinterpret_cast<const float2*>(p.beta + col));
   const int rows = min(32, p.M - row0);
 #pragma unroll 8
   for (int r = 0; r < 32; ++r) {
-    const float2 x = *reinterpret_cast<const float2*>(stage + r * LDS + lane * 2);
+    const float2 x = *reinterpret_cast<const float2*>(stage + acc_idx<64>(r, lane * 2));
     const float mean = __shfl_sync(0xffffffffu, mean_l, r), rstd = __shfl_sync(0xffffffffu, rstd_l, r);
     if (r < rows)
       *reinterpret_cast<__half2*>(p.out_h + (size_t)(row0 + r) * p.out_h_ld + col) =
@@ -314,7 +324,6 @@ __device__ __forceinline__ void ld8h(const __half* p, float (&v)[8]) {
 template <int EPI, int W, int ACT>
 __device__ __forceinline__ void epilogue_rows_impl(const GemmParams& p, int g, int row0, int lane, int col_base,
                                                    const float* __restrict__ stage, float mean_l, float rstd_l) {
-  constexpr int LDS = W + 4;
   constexpr int LPR = W / 8;             // lanes per row
   constexpr int RPS = 32 / LPR;          // rows per step
   constexpr int STEPS = 32 / RPS;
@@ -360,7 +369,11 @@ __device__ __forceinline__ void epilogue_rows_impl(const GemmParams& p, int g, i
       const int r = (s0 + u) * RPS + rsub;
       const size_t m = (size_t)(row0 + r);
       live[u] = r < rows;
-      ld8(stage + r * LDS + seg * 8, v[u]);
+      {
+        const float4 a = *reinterpret_cast<const float4*>(stage + acc_idx<W>(r, seg * 8));
+        const float4 b = *reinterpret_cast<const float4*>(stage + acc_idx<W>(r, seg * 8 + 4));
+        v[u][0] = a.x; v[u][1] = a.y; v[u][2] = a.z; v[u][3] = a.w; v[u][4] = b.x; v[u][5] = b.y; v[u][6] = b.z; v[u][7] = b.w;
+      }
       pos[u] = __shfl_sync(0xffffffffu, my_pos, r);
       orow[u] = __shfl_sync(0xffffffffu, my_orow, r);
       valid[u] = __shfl_sync(0xffffffffu, my_valid, r) != 0;

@@ -234,37 +234,55 @@ int sm_count() {
 
 // Persistent instantiations get one CTA per SM (fewer if there are fewer tiles); the one-tile-per-CTA ones one CTA per
 // tile.  EPI_RESID_LN: each row of tiles (gemm_tile keeps it consecutive) forms one thread-block cluster, which
-// exchanges row statistics through DSMEM.
-template <int BN, int EPI, int STAGES, bool PERSISTENT>
+// exchanges row statistics through DSMEM.  PAIR: two-CTA clusters, as many as can be resident at once (fewer if there
+// are fewer tile pairs).  That count comes from the occupancy API, not from SMs / 2: a cluster's CTAs share a GPC, and
+// a GPC with an odd number of free SMs leaves one idle; a grid beyond the resident clusters would run a second wave.
+template <int BN, int EPI, int STAGES, bool PERSISTENT, bool PAIR = false>
 static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream,
                      const OutMaps& om = no_out_maps()) {
   static unsigned long long attr_mask = 0;
+  static int max_clusters[64] = {0};
   constexpr int smem = gemm_smem_bytes<BN, EPI, STAGES, PERSISTENT>();
-  if (first_use_on_device(attr_mask)) {
-    MK_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, STAGES, PERSISTENT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  }
-  const int tiles = gemm_tile_count<BN>(p);
+  auto kernel = gemm_tc_kernel<BN, EPI, STAGES, PERSISTENT, PAIR>;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(PERSISTENT ? std::min(tiles, sm_count()) : tiles);
   cfg.blockDim = dim3(gemm_threads<PERSISTENT>()); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   int n_attr = 0;
+  if constexpr (EPI == EPI_RESID_LN || PAIR) {
+    attr[n_attr].id = cudaLaunchAttributeClusterDimension;
+    attr[n_attr].val.clusterDim.x = PAIR ? 2 : p.N / BN; attr[n_attr].val.clusterDim.y = 1; attr[n_attr++].val.clusterDim.z = 1;
+  }
+  cfg.attrs = attr;
+  cfg.numAttrs = n_attr;
+  int dev = 0;
+  if constexpr (PAIR) cudaGetDevice(&dev);
+  if (first_use_on_device(attr_mask)) {
+    MK_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    if constexpr (PAIR) {
+      cfg.gridDim = dim3(2 * sm_count());
+      MK_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&max_clusters[dev & 63], kernel, &cfg));
+    }
+  }
+  const int tiles = gemm_tile_count<BN>(p);
+  if constexpr (PAIR) {
+    const int n_clusters = max_clusters[dev & 63];
+    if (n_clusters <= 0) { set_last_error("GEMM: no two-CTA cluster of %d bytes of shared memory fits on this device", smem); return MK_ERR_UNSUPPORTED; }
+    cfg.gridDim = dim3(2 * std::min(gemm_tile_count<BN, 2>(p), n_clusters));
+  } else {
+    cfg.gridDim = dim3(PERSISTENT ? std::min(tiles, sm_count()) : tiles);
+  }
   if (pdl_enabled()) {
     attr[n_attr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[n_attr++].val.programmaticStreamSerializationAllowed = 1;
   }
-  if constexpr (EPI == EPI_RESID_LN) {
-    attr[n_attr].id = cudaLaunchAttributeClusterDimension;
-    attr[n_attr].val.clusterDim.x = p.N / BN; attr[n_attr].val.clusterDim.y = 1; attr[n_attr++].val.clusterDim.z = 1;
-  }
-  cfg.attrs = attr;
   cfg.numAttrs = n_attr;
-  MK_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, EPI, STAGES, PERSISTENT>, tmA, tmB, p, om));
+  MK_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, p, om));
   return MK_OK;
 }
 
 // Grids of at most ~1.25 tiles per SM run one tile per CTA on a deep ring (more bytes in flight per tile).  Grids of more
-// than 8 tiles per SM run the persistent kernel: every ViT-B GEMM and head GEMM of the 32-pair batch (>= 1060 M-tiles).
+// than 8 tiles per SM run the persistent kernel on CTA pairs that share each B tile: every ViT-B GEMM and head GEMM of
+// the 32-pair batch (>= 1060 M-tiles).
 // The ones in between run one tile per CTA with two CTAs per SM: every GEMM of a single ViT-S pair (at most 544 tiles),
 // where the persistent kernel measured slower.
 static bool deep_ring(int tiles, const GemmParams& p) {
@@ -287,6 +305,18 @@ static int launch_one(const GemmOperand& A, const GemmOperand& B, const GemmPara
     CUtensorMap tmA, tmB;
     int rc = make_tensor_map_f16(&tmA, A.ptr, A.rows, A.cols, A.ld, BLOCK_M);
     if (rc) return rc;
+    if constexpr (persistent_epilogue<EPI>()) {
+      // the persistent kernel: CTA pairs that share B (each loads half of the B box), unless the test / benchmark
+      // selection asks for the unpaired kernel
+      const bool forced = impl == GEMM_IMPL_TC_PAIRED || impl == GEMM_IMPL_TC_UNPAIRED;
+      if (forced || persistent_grid(tiles)) {
+        const bool pair = impl != GEMM_IMPL_TC_UNPAIRED;
+        rc = make_tensor_map_f16(&tmB, B.ptr, B.rows, B.cols, B.ld, pair ? BN / 2 : BN);
+        if (rc) return rc;
+        if (pair) return launch_tc<BN, EPI, ring_stages<BN>(), true, true>(tmA, tmB, p, stream);
+        return launch_tc<BN, EPI, ring_stages<BN>(), true>(tmA, tmB, p, stream);
+      }
+    }
     rc = make_tensor_map_f16(&tmB, B.ptr, B.rows, B.cols, B.ld, BN);
     if (rc) return rc;
     if constexpr (EPI == EPI_DUAL) {
@@ -300,8 +330,6 @@ static int launch_one(const GemmOperand& A, const GemmOperand& B, const GemmPara
       }
     }
     if (deep_ring(tiles, p)) return launch_tc<BN, EPI, deep_stages<BN>(), false>(tmA, tmB, p, stream);
-    if constexpr (persistent_epilogue<EPI>())
-      if (persistent_grid(tiles)) return launch_tc<BN, EPI, ring_stages<BN>(), true>(tmA, tmB, p, stream);
     return launch_tc<BN, EPI, shallow_stages<BN>(), false>(tmA, tmB, p, stream);
   }
   MK_CUDA_CHECK(cudaGetLastError());

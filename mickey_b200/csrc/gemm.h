@@ -9,7 +9,10 @@ struct GemmOperand {       // a row-major fp16 matrix [rows, cols] with leading 
   long long rows, cols, ld;
 };
 
-enum GemmImpl : int { GEMM_IMPL_DEFAULT = 0, GEMM_IMPL_TC = 1, GEMM_IMPL_SIMT = 2 };
+// GEMM_IMPL_TC_PAIRED / _UNPAIRED run the persistent kernel with or without two-CTA pairs on every grid whose epilogue
+// it serves (other epilogues run as GEMM_IMPL_TC), whatever the grid size: a test or a benchmark can set the two side
+// by side.  The default picks the paired kernel for grids of more than 8 tiles per SM.
+enum GemmImpl : int { GEMM_IMPL_DEFAULT = 0, GEMM_IMPL_TC = 1, GEMM_IMPL_SIMT = 2, GEMM_IMPL_TC_PAIRED = 3, GEMM_IMPL_TC_UNPAIRED = 4 };
 
 int make_tensor_map_f16(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld_elems, int box_rows);
 // Uncached TMA load map of a row-major fp16 or fp32 [rows, cols] operand with leading dimension ld_elems: box = 128 bytes

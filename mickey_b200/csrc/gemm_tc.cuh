@@ -11,7 +11,9 @@
 // over from tile to tile, so the next tile's loads are in flight while the current one is still in its MMAs.  When a
 // tile's K loop has drained, the MMA warpgroups park the accumulators in a staging buffer outside the ring, as eight
 // 32 x (BN/2) blocks (the layout epilogue_rows reads), and go on to the next tile while the epilogue warps run
-// tile_epilogue from the staged blocks.
+// tile_epilogue from the staged blocks.  The default persistent launch (PAIR) runs two-CTA clusters on M-adjacent tiles
+// that share each B tile through TMA multicast (see the kernel), which cuts the L2-to-SM bytes per chunk from 32 KB to
+// 24 KB (BN = 128).
 //
 // The other instantiations (!PERSISTENT) run one tile per CTA (grid = tiles, the same loop runs once) with 288 threads:
 // the MMA warps park the accumulators in the idle ring and run the epilogue themselves, warp 8 is the producer.  They
@@ -50,7 +52,7 @@ constexpr int DUAL_STAGE_BYTES = 3 * 4096;
 constexpr int DUAL_AUX_BYTES = 8 * 64 * 4;
 constexpr int DUAL_BYTES = 8 * DUAL_STAGE_BYTES + DUAL_AUX_BYTES;
 
-template <int BN> constexpr int acc_block_floats() { return 32 * (BN / 2 + 4); }   // one warp's 32 x (BN/2) block, ld BN/2 + 4
+template <int BN> constexpr int acc_block_floats() { return 32 * (BN / 2); }   // one warp's 32 x (BN/2) block (acc_idx layout)
 template <int BN> constexpr int acc_tile_bytes() { return 8 * acc_block_floats<BN>() * 4; }
 template <int BN, int STAGES> constexpr int ring_bytes() { return STAGES * (BLOCK_M * BLOCK_K * 2 + BN * BLOCK_K * 2); }
 // Persistent: the accumulator staging buffer follows the ring.  One tile per CTA: after the K loop the ring region
@@ -80,20 +82,22 @@ template <int BN, int EPI, int STAGES, bool PERSISTENT> constexpr int gemm_ctas_
 // 50 MB L2 while all of B is a few MB: the ~132 tiles in flight at once then cover a few complete rows of tiles, every
 // A row-panel is read from HBM about once and B stays resident in L2.  An M-fastest order would instead stream A once
 // per column of N-tiles.  EPI_RESID_LN relies on a row of tiles being consecutive: its clusters are those rows.
+// MT = 2 (the paired persistent kernel) walks the same order over pairs of M-tiles 2 mp, 2 mp + 1: the CTA of cluster
+// rank r takes M-tile 2 mp + r.  With an odd M-tile count the last pair's rank-1 tile starts at or beyond M.
 struct GemmTile { int g, m0, n0, n_tile; };
-template <int BN>
+template <int BN, int MT = 1>
 __host__ __device__ __forceinline__ int gemm_tile_count(const GemmParams& p) {
-  return ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BN - 1) / BN) * p.groups;
+  return ((p.M + MT * BLOCK_M - 1) / (MT * BLOCK_M)) * ((p.N + BN - 1) / BN) * p.groups;
 }
-template <int BN>
-__device__ __forceinline__ GemmTile gemm_tile(const GemmParams& p, int t) {
-  const int n_tiles = (p.N + BN - 1) / BN, m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+template <int BN, int MT = 1>
+__device__ __forceinline__ GemmTile gemm_tile(const GemmParams& p, int t, int rank = 0) {
+  const int n_tiles = (p.N + BN - 1) / BN, m_units = (p.M + MT * BLOCK_M - 1) / (MT * BLOCK_M);
   const int n = t % n_tiles;
   t /= n_tiles;
   int g, m;
   if (p.a_row_group_off == 0 && p.a_col_group_off == 0) { g = t % p.groups; m = t / p.groups; }
-  else { m = t % m_tiles; g = t / m_tiles; }
-  return {g, m * BLOCK_M, n * BN, n};
+  else { m = t % m_units; g = t / m_units; }
+  return {g, (m * MT + rank) * BLOCK_M, n * BN, n};
 }
 
 // ---- PTX wrappers ------------------------------------------------------------------------------------
@@ -123,6 +127,24 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
+}
+// The same box written to offset `dst` of every CTA of the cluster in `cta_mask`; each destination's mbarrier at offset
+// `bar` receives the box's bytes.
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask) : "memory");
+}
+// arrive on the mbarrier at offset `bar` of CTA `cta_rank` of the cluster (this CTA's own rank included).  The default
+// .release.cta semantics: a .cluster-scoped release costs a MEMBAR.GPU per arrival (measured 3x slower GEMMs), and the
+// only accesses it would order are the wgmma reads of the stage, which have retired (wgmma.wait_group) before the arrival.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta_rank) {
+  asm volatile(
+      "{\n\t.reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t}"
+      ::"r"(bar), "r"(cta_rank) : "memory");
 }
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
@@ -211,10 +233,10 @@ __device__ __forceinline__ float ld_dsmem_f32(uint32_t local_smem_addr, uint32_t
 template <int BN>
 __device__ __forceinline__ void acc_chunk(const float* acc, int q, int lane, int c, float (&v)[32]) {
   constexpr int W = BN / 2;
-  const float4* src = reinterpret_cast<const float4*>(acc + (q + 4 * ((c * 32) / W)) * acc_block_floats<BN>() + lane * (W + 4) + (c * 32) % W);
+  const float* blk = acc + (q + 4 * ((c * 32) / W)) * acc_block_floats<BN>();
 #pragma unroll
   for (int k4 = 0; k4 < 8; ++k4) {
-    const float4 t = src[k4];
+    const float4 t = *reinterpret_cast<const float4*>(blk + acc_idx<W>(lane, (c * 32) % W + 4 * k4));
     v[k4 * 4] = t.x; v[k4 * 4 + 1] = t.y; v[k4 * 4 + 2] = t.z; v[k4 * 4 + 3] = t.w;
   }
 }
@@ -326,7 +348,13 @@ __device__ __forceinline__ void tile_epilogue(const GemmParams& p, const OutMaps
 }
 
 // ---- kernel ------------------------------------------------------------------------------------------
-template <int BN, int EPI, int STAGES, bool PERSISTENT>
+// PAIR (persistent only): the grid is made of two-CTA clusters.  Both CTAs of a cluster walk the same (group, N-tile)
+// sequence on M-tiles 2 mp and 2 mp + 1 (gemm_tile<BN, 2>), so they read the same B tile in every K chunk.  Each
+// CTA's producer loads its own A box and one half of the B box (BN/2 rows; tmB is encoded with that box), multicast
+// into stage s of both CTAs; each CTA's full barrier still expects STAGE_BYTES.  A stage is refilled only when the
+// MMA warps of both CTAs have released it: every MMA warp arrives on the empty barrier of both CTAs (16 arrivals per
+// phase).  The MMAs, their operands and their K order are those of the unpaired kernel, so the outputs are identical.
+template <int BN, int EPI, int STAGES, bool PERSISTENT, bool PAIR = false>
 __global__ void __launch_bounds__((gemm_threads<PERSISTENT>()), (gemm_ctas_per_sm<BN, EPI, STAGES, PERSISTENT>()))
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p,
                const __grid_constant__ OutMaps om) {
@@ -338,8 +366,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int W = BN / 2;
   static_assert(!PERSISTENT || persistent_epilogue<EPI>(), "this epilogue runs one tile per CTA");
+  static_assert(!PAIR || PERSISTENT, "CTA pairs: persistent kernel only");
   constexpr bool ONE_TILE = !PERSISTENT;
   constexpr int WARP_TMA = gemm_warp_tma<PERSISTENT>();
+  constexpr int MT = PAIR ? 2 : 1;                              // M-tiles per unit of work
+  // a pair's two CTAs are blockIdx.x 2c and 2c + 1 (cluster c, rank blockIdx.x & 1)
+  const int rank = PAIR ? (int)(blockIdx.x & 1) : 0;
+  const int work0 = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+  const int work_step = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // swizzle-128B tiles need 1024-byte alignment
@@ -355,20 +389,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n_tiles_total = gemm_tile_count<BN>(p);
+  const int n_work = gemm_tile_count<BN, MT>(p);
 
   if (warp == WARP_TMA && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar0 + 8 * s, 1);
-      mbar_init(empty_bar0 + 8 * s, 8);            // one arrive per MMA warp
+      mbar_init(empty_bar0 + 8 * s, 8 * MT);       // one arrive per MMA warp (of both CTAs of a pair)
     }
     mbar_init(acc_full_bar, 256);
     mbar_init(acc_empty_bar, 256);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  // a pair: the peer's barriers must be initialised before this CTA's multicasts or remote arrivals reach them
+  if constexpr (PAIR) cluster_sync_all();
+  else __syncthreads();
   pdl_wait();                    // everything above touched no global memory; operands of the previous kernel are now visible
 
   if (warp >= WARP_TMA) {
@@ -377,8 +413,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (warp == WARP_TMA && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x) {
-        const GemmTile tile = gemm_tile<BN>(p, t);
+      for (int t = work0; t < n_work; t += work_step) {
+        const GemmTile tile = gemm_tile<BN, MT>(p, t, rank);
         const int a_col0 = p.a_col_base + tile.g * p.a_col_group_off;
         const int a_row0 = tile.m0 + tile.g * p.a_row_group_off;
         const int b_row0 = tile.n0 + tile.g * p.b_row_group_off;
@@ -390,7 +426,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           const uint32_t fb = full_bar0 + 8 * stage;
           mbar_expect_tx(fb, STAGE_BYTES);
           tma_load_2d(sa, &tmA, fb, a_col0 + kin * BLOCK_K, a_row0 + p.tap_shift[tap]);
-          tma_load_2d(sa + A_BYTES, &tmB, fb, kc * BLOCK_K, b_row0);
+          // B rows of a half box are a multiple of 8 (1024 bytes), so the halves keep the 128-byte swizzle pattern
+          if constexpr (PAIR) tma_load_2d_multicast(sa + A_BYTES + rank * (B_BYTES / 2), &tmB, fb, kc * BLOCK_K, b_row0 + rank * (BN / 2), 0x3);
+          else tma_load_2d(sa + A_BYTES, &tmB, fb, kc * BLOCK_K, b_row0);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -399,6 +437,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     pdl_trigger();
     // EPI_RESID_LN: every thread of every CTA of the cluster takes part in the three cluster barriers
     if constexpr (EPI == EPI_RESID_LN) { cluster_sync_all(); cluster_sync_all(); cluster_sync_all(); }
+    // a pair: no CTA may exit while its peer can still multicast into its ring or arrive on its barriers
+    if constexpr (PAIR) cluster_sync_all();
     return;
   }
 
@@ -407,7 +447,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int wg = warp >> 2;
     int stage = 0;
     uint32_t phase = 0, acc_phase = 0;
-    for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x) {
+    // release a ring stage to the producer(s) that fill it
+    auto release = [&](int s) {
+      if constexpr (PAIR) { mbar_arrive_cluster(empty_bar0 + 8 * s, 0); mbar_arrive_cluster(empty_bar0 + 8 * s, 1); }
+      else mbar_arrive(empty_bar0 + 8 * s);
+    };
+    for (int t = work0; t < n_work; t += work_step) {
       float d[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
@@ -424,13 +469,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         wgmma_commit();
         wgmma_wait<1>();                               // the previous chunk's MMAs have retired: release its stage
         reg_fence(d);
-        if (kc > 0 && lane == 0) mbar_arrive(empty_bar0 + 8 * (stage == 0 ? STAGES - 1 : stage - 1));
+        if (kc > 0 && lane == 0) release(stage == 0 ? STAGES - 1 : stage - 1);
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
       reg_fence(d);
-      if (lane == 0) mbar_arrive(empty_bar0 + 8 * (stage == 0 ? STAGES - 1 : stage - 1));
-      if (t + (int)gridDim.x >= n_tiles_total) pdl_trigger();   // last K loop done: the next kernel may start its prologue
+      if (lane == 0) release(stage == 0 ? STAGES - 1 : stage - 1);
+      if (t + work_step >= n_work) pdl_trigger();   // last K loop done: the next kernel may start its prologue
 
       // ===== hand the accumulators to the epilogue through the staging buffer =====
       if constexpr (ONE_TILE) consumer_sync();      // the staging buffer is the ring: both warpgroups are done reading it
@@ -442,7 +487,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int r = r_base + 8 * h, c = 8 * j + 2 * (lane & 3);
-          float* dst = acc + ((r >> 5) + 4 * (c / W)) * acc_block_floats<BN>() + (r & 31) * (W + 4) + (c % W);
+          float* dst = acc + ((r >> 5) + 4 * (c / W)) * acc_block_floats<BN>() + acc_idx<W>(r & 31, c % W);
           *reinterpret_cast<float2*>(dst) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
         }
       }
@@ -459,6 +504,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
     if constexpr (EPI == EPI_DUAL) { if (p.out_tma && lane == 0) tma_store_wait_all(); }   // smem must outlive the bulk reads
+    if constexpr (PAIR) cluster_sync_all();
     return;
   }
 
@@ -467,17 +513,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   setmaxnreg_inc<GEMM_REGS_EPILOGUE>();
   const int ew = warp - GEMM_WARP_EPI;
   uint32_t acc_phase = 0;
-  for (int t = blockIdx.x; t < n_tiles_total; t += gridDim.x) {
-    const GemmTile tile = gemm_tile<BN>(p, t);
+  for (int t = work0; t < n_work; t += work_step) {
+    const GemmTile tile = gemm_tile<BN, MT>(p, t, rank);
     mbar_wait(acc_full_bar, acc_phase);
-    if (t + (int)gridDim.x >= n_tiles_total) pdl_trigger();
-    tile_epilogue<BN, EPI>(p, om, tile.g, tile.m0, tile.n0, tile.n_tile, ew & 3, ew >> 2, lane, acc,
-                           reinterpret_cast<float*>(smem_raw + (red_saddr - raw)), red_saddr,
-                           reinterpret_cast<float*>(gbase + ew * DUAL_STAGE_BYTES),
-                           reinterpret_cast<float*>(gbase + 8 * DUAL_STAGE_BYTES) + ew * 64);
+    if (t + work_step >= n_work) pdl_trigger();
+    // the rank-1 tile of the last pair of an odd M-tile count lies wholly beyond M: it stores nothing
+    if (tile.m0 < p.M)
+      tile_epilogue<BN, EPI>(p, om, tile.g, tile.m0, tile.n0, tile.n_tile, ew & 3, ew >> 2, lane, acc,
+                             reinterpret_cast<float*>(smem_raw + (red_saddr - raw)), red_saddr,
+                             reinterpret_cast<float*>(gbase + ew * DUAL_STAGE_BYTES),
+                             reinterpret_cast<float*>(gbase + 8 * DUAL_STAGE_BYTES) + ew * 64);
     mbar_arrive(acc_empty_bar);
     acc_phase ^= 1;
   }
+  if constexpr (PAIR) cluster_sync_all();
 }
 
 }  // namespace mk
