@@ -411,10 +411,43 @@ class Engine(_lib.Handle):
             n_img, _, H, W = images.shape
         return images, u8, n_img, H, W
 
-    def _outputs_of_extract(self, n_img, N):
+    def _nn_outputs(self, B, N, lean):
+        """(scores, kp_scores, final_scores) of B pairs as nn_empty views; scores and kp_scores are None when lean."""
         dev = self.device
-        return (torch.empty(n_img, 2, N, device=dev), torch.empty(n_img, 1, N, device=dev), torch.empty(n_img, 1, N, device=dev),
-                torch.empty(n_img, self.mkcfg.desc_dim, N, device=dev))
+        return (None if lean else nn_empty(B, N, dev)), (None if lean else nn_empty(B, N, dev)), nn_empty(B, N, dev)
+
+    def _solver_outputs(self, B):
+        dev, c = self.device, self.mkcfg
+        return {"pose": torch.empty(B, 13, device=dev), "best_set": torch.empty(B, dtype=torch.int32, device=dev),
+                "inlier_mask": torch.empty(B, c.num_sampled, device=dev),
+                "sampled_idx": torch.empty(B * c.it_matches, c.num_sampled, dtype=torch.int32, device=dev),
+                "status": torch.zeros(1, dtype=torch.int32, device=dev)}
+
+    def _outputs(self, n_img, n_pairs, N, lean=False, scr_dsc=True):
+        """Fresh outputs of a call on n_img images and n_pairs pairs, keyed as forward() returns them: kps, depth and (with
+        scr_dsc) scr, dsc per image; when n_pairs > 0, the matcher's and the solver's outputs."""
+        dev = self.device
+        out = {"kps": torch.empty(n_img, 2, N, device=dev), "depth": torch.empty(n_img, 1, N, device=dev)}
+        if scr_dsc:
+            out.update(scr=torch.empty(n_img, 1, N, device=dev), dsc=torch.empty(n_img, self.mkcfg.desc_dim, N, device=dev))
+        if n_pairs:
+            out["scores"], out["kp_scores"], out["final_scores"] = self._nn_outputs(n_pairs, N, lean)
+            out.update(self._solver_outputs(n_pairs))
+        return out
+
+    @staticmethod
+    def _output_args(out):
+        """The trailing outputs of mk_forward / mk_forward_u8 (with scr, dsc) or mk_forward_pairs, in the header's order."""
+        p, f = _lib.ptr, out["final_scores"]
+        return (*(p(out[k]) for k in ("kps", "depth", "scr", "dsc", "scores", "kp_scores") if k in out), p(f), f.stride(1),
+                *(p(out[k]) for k in ("pose", "best_set", "inlier_mask", "sampled_idx", "status")))
+
+    @staticmethod
+    def _forward_seed(seed):
+        return (int(seed) & (2 ** 64 - 1)) or 1         # a seed of 0 would continue the device-side sequence
+
+    def _intrinsics(self, K):
+        return K.to(self.device, torch.float32).contiguous()
 
     def extract(self, images: torch.Tensor):
         """images fp32 [2B, 3, H, W] (image0 batch then image1 batch) -> kps, depth, scr, dsc.
@@ -424,12 +457,12 @@ class Engine(_lib.Handle):
         assert n_img % 2 == 0
         B, N = n_img // 2, (H // PATCH) * (W // PATCH)
         ws = self._ws_for(B, H, W)
-        kps, depth, scr, dsc = self._outputs_of_extract(n_img, N)
+        feats = tuple(self._outputs(n_img, 0, N).values())          # kps, depth, scr, dsc
         fn = self.lib.mk_extract_u8 if u8 else self.lib.mk_extract
         with self._ordered():
-            _lib.check(fn(self.h, _lib.ptr(images), B, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
-                          _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), _lib.stream()), "mk_extract")
-        return kps, depth, scr, dsc
+            _lib.check(fn(self.h, _lib.ptr(images), B, H, W, *map(_lib.ptr, feats), _lib.ptr(ws), ws.numel(), _lib.stream()),
+                       "mk_extract")
+        return feats
 
     # -- feature banks: extract images once, then match / solve any pairs among them ------------------------------
     def _bank_ws(self, n_img, n_pairs, H, W):
@@ -450,12 +483,12 @@ class Engine(_lib.Handle):
         N = (H // PATCH) * (W // PATCH)
         self._use_geometry(H, W)
         ws = self._bank_ws(n_img, 0, H, W)
-        kps, depth, scr, dsc = self._outputs_of_extract(n_img, N)
+        feats = tuple(self._outputs(n_img, 0, N).values())          # kps, depth, scr, dsc
         fn = self.lib.mk_extract_images_u8 if u8 else self.lib.mk_extract_images
         with self._ordered():
-            _lib.check(fn(self.h, _lib.ptr(images), n_img, H, W, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(scr),
-                          _lib.ptr(dsc), _lib.ptr(ws), ws.numel(), _lib.stream()), "mk_extract_images")
-        return kps, depth, scr, dsc
+            _lib.check(fn(self.h, _lib.ptr(images), n_img, H, W, *map(_lib.ptr, feats), _lib.ptr(ws), ws.numel(),
+                          _lib.stream()), "mk_extract_images")
+        return feats
 
     def forward_pairs(self, bank0, idx0, bank1, idx1, K0, K1, seed: int, image_size, lean: bool = False):
         """Match and solve the pairs (bank0[idx0[p]], bank1[idx1[p]]) in one C call (mk_forward_pairs).
@@ -468,31 +501,19 @@ class Engine(_lib.Handle):
         self._use_geometry(H, W)
         P, N = idx0.numel(), bank0[0].shape[-1]
         ws = self._bank_ws(0, P, H, W)
-        dev, c = self.device, self.mkcfg
-        out = {"kps": torch.empty(2 * P, 2, N, device=dev), "depth": torch.empty(2 * P, 1, N, device=dev),
-               "scores": None if lean else nn_empty(P, N, dev), "kp_scores": None if lean else nn_empty(P, N, dev),
-               "final_scores": nn_empty(P, N, dev), "pose": torch.empty(P, 13, device=dev),
-               "best_set": torch.empty(P, dtype=torch.int32, device=dev), "inlier_mask": torch.empty(P, c.num_sampled, device=dev),
-               "sampled_idx": torch.empty(P * c.it_matches, c.num_sampled, dtype=torch.int32, device=dev),
-               "status": torch.zeros(1, dtype=torch.int32, device=dev)}
-        K0 = K0.to(dev, torch.float32).contiguous()
-        K1 = K1.to(dev, torch.float32).contiguous()
-        seed = (int(seed) & (2 ** 64 - 1)) or 1
+        out = self._outputs(2 * P, P, N, lean, scr_dsc=False)
+        K0, K1 = self._intrinsics(K0), self._intrinsics(K1)
         p = _lib.ptr
         with self._ordered():
             _lib.check(self.lib.mk_forward_pairs(
                 self.h, *(p(t) for t in bank0), bank0[0].shape[0], *(p(t) for t in bank1), bank1[0].shape[0], p(idx0), p(idx1),
-                p(K0), p(K1), P, C.c_ulonglong(seed), p(out["kps"]), p(out["depth"]), p(out["scores"]), p(out["kp_scores"]),
-                p(out["final_scores"]), out["final_scores"].stride(1), p(out["pose"]), p(out["best_set"]), p(out["inlier_mask"]),
-                p(out["sampled_idx"]), p(out["status"]), p(ws), ws.numel(), _lib.stream()), "mk_forward_pairs")
+                p(K0), p(K1), P, C.c_ulonglong(self._forward_seed(seed)), *self._output_args(out), p(ws), ws.numel(),
+                _lib.stream()), "mk_forward_pairs")
         return out
 
     def match(self, B: int, N: int, lean: bool = False):
         """lean: only final_scores (the matrix the solver reads) is materialised; scores / kp_scores come back as None."""
-        dev = self.device
-        scores = None if lean else nn_empty(B, N, dev)
-        kp_scores = None if lean else nn_empty(B, N, dev)
-        final = nn_empty(B, N, dev)
+        scores, kp_scores, final = self._nn_outputs(B, N, lean)
         with self._ordered():
             _lib.check(self.lib.mk_match(self.h, B, _lib.ptr(scores), _lib.ptr(kp_scores), _lib.ptr(final), final.stride(1),
                                          _lib.ptr(self.ws), self.ws.numel(), _lib.stream()), "mk_match")
@@ -500,29 +521,15 @@ class Engine(_lib.Handle):
 
     # -- whole path in one C call, optionally replayed from a CUDA graph -------------------------------------------
     def _static_buffers(self, B, H, W, u8=False, lean=False):
-        dev, c = self.device, self.mkcfg
-        N = (H // PATCH) * (W // PATCH)
-        f = lambda *s: torch.empty(*s, device=dev)                       # noqa: E731
-        return {
-            "images": torch.empty(2 * B, H, W, 3, dtype=torch.uint8, device=dev) if u8 else f(2 * B, 3, H, W),
-            "K0": f(B, 3, 3), "K1": f(B, 3, 3),
-            "kps": f(2 * B, 2, N), "depth": f(2 * B, 1, N), "scr": f(2 * B, 1, N), "dsc": f(2 * B, c.desc_dim, N),
-            "scores": None if lean else nn_empty(B, N, dev), "kp_scores": None if lean else nn_empty(B, N, dev),
-            "final_scores": nn_empty(B, N, dev), "pose": f(B, 13),
-            "best_set": torch.empty(B, dtype=torch.int32, device=dev), "inlier_mask": f(B, c.num_sampled),
-            "sampled_idx": torch.empty(B * c.it_matches, c.num_sampled, dtype=torch.int32, device=dev),
-            "status": torch.zeros(1, dtype=torch.int32, device=dev),
-        }
+        dev = self.device
+        images = torch.empty(2 * B, H, W, 3, dtype=torch.uint8, device=dev) if u8 else torch.empty(2 * B, 3, H, W, device=dev)
+        return {"images": images, "K0": torch.empty(B, 3, 3, device=dev), "K1": torch.empty(B, 3, 3, device=dev),
+                **self._outputs(2 * B, B, (H // PATCH) * (W // PATCH), lean)}
 
     def _call_forward(self, st, B, H, W, seed):
-        ws = self.ws
         fn = self.lib.mk_forward_u8 if st["images"].dtype == torch.uint8 else self.lib.mk_forward
-        _lib.check(fn(
-            self.h, _lib.ptr(st["images"]), _lib.ptr(st["K0"]), _lib.ptr(st["K1"]), B, H, W, C.c_ulonglong(seed),
-            _lib.ptr(st["kps"]), _lib.ptr(st["depth"]), _lib.ptr(st["scr"]), _lib.ptr(st["dsc"]), _lib.ptr(st["scores"]),
-            _lib.ptr(st["kp_scores"]), _lib.ptr(st["final_scores"]), st["final_scores"].stride(1), _lib.ptr(st["pose"]), _lib.ptr(st["best_set"]),
-            _lib.ptr(st["inlier_mask"]), _lib.ptr(st["sampled_idx"]), _lib.ptr(st["status"]), _lib.ptr(ws), ws.numel(),
-            _lib.stream()), "mk_forward")
+        _lib.check(fn(self.h, _lib.ptr(st["images"]), _lib.ptr(st["K0"]), _lib.ptr(st["K1"]), B, H, W, C.c_ulonglong(seed),
+                      *self._output_args(st), _lib.ptr(self.ws), self.ws.numel(), _lib.stream()), "mk_forward")
 
     def forward(self, image0, image1, K0, K1, seed: int, use_graph: bool = True, lean: bool = False):
         """Whole hot path (extract -> match -> solve) for a batch of pairs.
@@ -611,7 +618,7 @@ class Engine(_lib.Handle):
         for d, s in zip(dst, ops):                      # device operands: in order behind the caller's stream (see forward)
             if s.device.type != "cpu":
                 d.copy_(s, non_blocking=True)
-        seed = (int(seed) & (2 ** 64 - 1)) or 1
+        seed = self._forward_seed(seed)
         if not use_graph:
             self._call_forward(st, B, H, W, seed)
         elif ent["graph"] is None and ent["calls"] == 0:
@@ -635,30 +642,22 @@ class Engine(_lib.Handle):
             ent["done"] = torch.cuda.Event()
         ent["done"].record(main)
 
-    def solve(self, final_scores, kps, depth, K0, K1, seed: int, outer_idx=None, inner_idx=None, want_extras=False):
+    def solve(self, final_scores, kps, depth, K0, K1, seed: int, outer_idx=None, inner_idx=None):
         """kps [2B,2,N], depth [2B,1,N] as produced by extract (image0 rows first).  final_scores [B,N,N] may be a padded
-        view (last dim contiguous, rows `stride(1)` floats apart) or any tensor (made contiguous)."""
+        view (last dim contiguous, rows `stride(1)` floats apart) or any tensor (made contiguous).  Returns the solver's
+        outputs (_solver_outputs) and hyp_scores [B, IT_MATCHES * IT_RANSAC].  A seed of 0 continues the device-side
+        sequence."""
         B, N, _ = final_scores.shape
         final_scores, pitch = _lib.pitched(final_scores)
-        dev = self.device
-        c = self.mkcfg
-        pose = torch.empty(B, 13, device=dev)
-        status = torch.zeros(1, dtype=torch.int32, device=dev)
-        best_set = torch.empty(B, dtype=torch.int32, device=dev) if want_extras else None
-        mask = torch.empty(B, c.num_sampled, device=dev) if want_extras else None
-        sampled = torch.empty(B * c.it_matches, c.num_sampled, dtype=torch.int32, device=dev) if want_extras else None
-        hyp = torch.empty(B, c.it_matches * c.it_ransac, device=dev) if want_extras else None
-        if outer_idx is not None:
-            outer_idx = outer_idx.to(dev, torch.int32).contiguous()
-        if inner_idx is not None:
-            inner_idx = inner_idx.to(dev, torch.int32).contiguous()
-        K0 = K0.to(dev, torch.float32).contiguous()
-        K1 = K1.to(dev, torch.float32).contiguous()
+        dev, c = self.device, self.mkcfg
+        out = self._solver_outputs(B)
+        out["hyp_scores"] = torch.empty(B, c.it_matches * c.it_ransac, device=dev)
+        outer_idx, inner_idx = (None if i is None else i.to(dev, torch.int32).contiguous() for i in (outer_idx, inner_idx))
+        K0, K1 = self._intrinsics(K0), self._intrinsics(K1)
+        p = _lib.ptr
         with self._ordered():
             _lib.check(self.lib.mk_solve_pose(
-                self.h, _lib.ptr(final_scores), pitch, _lib.ptr(kps), _lib.ptr(depth), _lib.ptr(K0), _lib.ptr(K1), B, N,
-                C.c_ulonglong(seed & (2 ** 64 - 1)), _lib.ptr(outer_idx), _lib.ptr(inner_idx), _lib.ptr(pose),
-                _lib.ptr(best_set), _lib.ptr(mask), _lib.ptr(sampled), _lib.ptr(hyp), _lib.ptr(status),
-                _lib.ptr(self.ws), self.ws.numel(), _lib.stream()), "mk_solve_pose")
-        return {"pose": pose, "status": status, "best_set": best_set, "inlier_mask": mask, "sampled_idx": sampled,
-                "hyp_scores": hyp}
+                self.h, p(final_scores), pitch, p(kps), p(depth), p(K0), p(K1), B, N, C.c_ulonglong(seed & (2 ** 64 - 1)),
+                p(outer_idx), p(inner_idx), p(out["pose"]), p(out["best_set"]), p(out["inlier_mask"]), p(out["sampled_idx"]),
+                p(out["hyp_scores"]), p(out["status"]), p(self.ws), self.ws.numel(), _lib.stream()), "mk_solve_pose")
+        return out

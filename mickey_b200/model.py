@@ -116,6 +116,50 @@ def synthetic_backbone_allowed() -> bool:
     return os.environ.get("MICKEY_SYNTHETIC_BACKBONE", "0") == "1"
 
 
+def _set_correspondences(data, kps, depth, scr, dsc, grid, down_factor, scores=None, kp_scores=None):
+    """The data-dict keys ComputeCorrespondences sets (compute_correspondences.py:52-92) for n pairs: kps [2n,2,N] and
+    depth [2n,1,N] hold the image-0 rows first; scr = (scr0, scr1) and dsc = (dsc0, dsc1), [n,.,N] each; scores and
+    kp_scores are left out when None (lean outputs).  Every tensor stored is the given tensor or a view of it."""
+    gh, gw = grid
+    n = kps.shape[0] // 2
+    data["kps0_shape"], data["kps1_shape"], data["down_factor"] = [gh, gw], [gh, gw], down_factor
+    data["depth0_map"], data["depth1_map"] = depth[:n].reshape(n, 1, gh, gw), depth[n:].reshape(n, 1, gh, gw)
+    data["kps0"], data["kps1"] = kps[:n], kps[n:]
+    data["depth_kp0"], data["depth_kp1"] = depth[:n], depth[n:]
+    data["scr0"], data["scr1"] = scr
+    data["dsc0"], data["dsc1"] = dsc
+    if scores is not None:
+        data["scores"], data["kp_scores"] = scores, kp_scores
+
+
+def _pose_views(pose):
+    """R [B,3,3], t [B,1,3] and the soft inlier count [B,1]: views of the solver's pose [B,13] = R row-major | t | inliers."""
+    B = pose.shape[0]
+    return pose[:, :9].reshape(B, 3, 3), pose[:, 9:12].reshape(B, 1, 3), pose[:, 12:13]
+
+
+def _inlier_list(solver, final_scores, kps0, kps1, depth_kp0, depth_kp1):
+    """The reference's inlier list (probabilisticProcrustes.py:305-327) from the solver's winning sampled set and its
+    hard-inlier mask: per pair, the rows [x0, y0, x1, y1, score, d0, d1] of the set's inlier cells, sorted by score
+    descending.  solver: best_set [B], sampled_idx [B*IT_MATCHES, S], inlier_mask [B, S] and status of the solver call.
+    Any zero-pose status bit (bits 0-2 from the solver, bit 3 from mk_forward_pairs' index check) gives every pair an
+    empty [0, 5] tensor."""
+    B, N = kps0.shape[0], final_scores.shape[-1]
+    if int(solver["status"].item()) & 15:
+        return [torch.zeros([0, 5]) for _ in range(B)]
+    cells = solver["sampled_idx"].long()[solver["best_set"].long()]           # [B, S]
+    mask = solver["inlier_mask"] > 0.5
+    i0, i1 = torch.div(cells, N, rounding_mode="trunc"), cells % N
+    bidx = torch.arange(B, device=cells.device)[:, None].expand_as(cells)
+    w = final_scores[bidx, i0, i1]
+    rows = torch.cat([kps0[bidx, :, i0], kps1[bidx, :, i1], w[..., None], depth_kp0[bidx, :, i0], depth_kp1[bidx, :, i1]], dim=-1)
+    out = []
+    for b in range(B):
+        rb = rows[b][mask[b]]
+        out.append(rb[torch.argsort(rb[:, 4], descending=True)])
+    return out
+
+
 class _ParamTree(nn.Module):
     """A module whose only job is to hold tensors under dotted names."""
 
@@ -168,40 +212,16 @@ class e2eProbabilisticProcrustesSolver:
     def estimate_pose_vectorized(self, batch, return_inliers=False, outer_idx=None, inner_idx=None, seed=None):
         eng = self._owner._engine()
         final = batch["final_scores"].detach().float()      # a padded-pitch view goes to the kernels as it is
-        B, N, _ = final.shape
         kps = torch.cat([batch["kps0"], batch["kps1"]], 0).detach().float().contiguous()
         depth = torch.cat([batch["depth_kp0"], batch["depth_kp1"]], 0).detach().float().contiguous()
         if seed is None:
             seed = int(torch.randint(1, 2 ** 62, (1,)).item())     # follows torch.manual_seed like the reference
-        res = eng.solve(final, kps, depth, batch["K_color0"], batch["K_color1"], seed, outer_idx=outer_idx,
-                        inner_idx=inner_idx, want_extras=True)
-        pose = res["pose"]
-        R = pose[:, :9].reshape(B, 3, 3).contiguous()
-        t = pose[:, 9:12].reshape(B, 1, 3).contiguous()
-        inliers = pose[:, 12:13].contiguous()
+        res = eng.solve(final, kps, depth, batch["K_color0"], batch["K_color1"], seed, outer_idx=outer_idx, inner_idx=inner_idx)
+        R, t, inliers = (v.contiguous() for v in _pose_views(res["pose"]))
         batch["_solver"] = res
         if not return_inliers:
             return R, t, inliers
-        # inlier list of the winning sampled set (probabilisticProcrustes.py:305-327): rows
-        # [x0, y0, x1, y1, score, d0, d1] sorted by score, assembled from the kernel's mask (plumbing only)
-        n_s = self.num_samples_matches
-        sets = res["best_set"].long()
-        cells = res["sampled_idx"].long()[sets]                           # [B, n_s]
-        mask = res["inlier_mask"] > 0.5
-        i0, i1 = torch.div(cells, N, rounding_mode="trunc"), cells % N
-        bidx = torch.arange(B, device=final.device)[:, None].expand(-1, n_s)
-        w = final[bidx, i0, i1]
-        rows = torch.cat([batch["kps0"][bidx, :, i0], batch["kps1"][bidx, :, i1], w[..., None],
-                          batch["depth_kp0"][bidx, :, i0], batch["depth_kp1"][bidx, :, i1]], dim=-1)
-        zero_pose = bool((res["status"].item() & 7) != 0)
-        out = []
-        for b in range(B):
-            if zero_pose:
-                out.append(torch.zeros([0, 5]))
-                continue
-            rb = rows[b][mask[b]]
-            out.append(rb[torch.argsort(rb[:, 4], descending=True)])
-        return R, t, inliers, out
+        return R, t, inliers, _inlier_list(res, final, batch["kps0"], batch["kps1"], batch["depth_kp0"], batch["depth_kp1"])
 
 
 class ComputeCorrespondences(nn.Module):
@@ -224,21 +244,10 @@ class ComputeCorrespondences(nn.Module):
                              "of a batch are extracted in one call)")
         images = torch.cat([im0, im1], dim=0)
         kps, depth, scr, dsc = eng.extract(images)
-        N = kps.shape[-1]
         H, W = eng.geo
-        gh, gw = H // PATCH, W // PATCH
-        scores, kp_scores, final = eng.match(B, N, lean=bool(getattr(self._owner, "lean_outputs", False)))
-        data["kps0_shape"], data["kps1_shape"] = [gh, gw], [gh, gw]
-        data["depth0_map"] = depth[:B].reshape(B, 1, gh, gw)
-        data["depth1_map"] = depth[B:].reshape(B, 1, gh, gw)
-        data["down_factor"] = self.down_factor
-        data["kps0"], data["kps1"] = kps[:B], kps[B:]
-        data["depth_kp0"], data["depth_kp1"] = depth[:B], depth[B:]
-        data["scr0"], data["scr1"] = scr[:B], scr[B:]
-        data["dsc0"], data["dsc1"] = dsc[:B], dsc[B:]
-        if scores is not None:
-            data["scores"] = scores
-            data["kp_scores"] = kp_scores
+        scores, kp_scores, final = eng.match(B, kps.shape[-1], lean=bool(getattr(self._owner, "lean_outputs", False)))
+        _set_correspondences(data, kps, depth, (scr[:B], scr[B:]), (dsc[:B], dsc[B:]), (H // PATCH, W // PATCH),
+                             self.down_factor, scores, kp_scores)
         data["_final_scores_fused"] = final
         return data["kps0"], data["dsc0"], data["kps1"], data["dsc1"]
 
@@ -342,24 +351,6 @@ class MickeyRelativePose(nn.Module):
         return self._eng
 
     # -- the hot path ------------------------------------------------------------------------------------------
-    def _inlier_list(self, data, st, B, N):
-        """probabilisticProcrustes.py:305-327 from the kernel's winning set + hard-inlier mask (plumbing)."""
-        n_s = self.e2e_Procrustes.num_samples_matches
-        cells = st["sampled_idx"].long()[st["best_set"].long()]
-        mask = st["inlier_mask"] > 0.5
-        i0, i1 = torch.div(cells, N, rounding_mode="trunc"), cells % N
-        bidx = torch.arange(B, device=cells.device)[:, None].expand(-1, n_s)
-        w = data["final_scores"][bidx, i0, i1]
-        rows = torch.cat([data["kps0"][bidx, :, i0], data["kps1"][bidx, :, i1], w[..., None],
-                          data["depth_kp0"][bidx, :, i0], data["depth_kp1"][bidx, :, i1]], dim=-1)
-        if int(st["status"].item()) & 15:                # any zero-pose status bit (bit 3: forward_pairs index out of range)
-            return [torch.zeros([0, 5])] * B
-        out = []
-        for b in range(B):
-            rb = rows[b][mask[b]]
-            out.append(rb[torch.argsort(rb[:, 4], descending=True)])
-        return out
-
     @torch.no_grad()
     def forward(self, data, return_inliers=False):
         """One C call (mk_forward) per batch, replayed from a CUDA graph after the first two calls.
@@ -382,25 +373,18 @@ class MickeyRelativePose(nn.Module):
         # the engine's copies into its fp32 input buffers, on the stream that also reads them
         st = eng.forward(im0, im1, data["K_color0"], data["K_color1"], seed,
                          use_graph=getattr(self, "use_graph", True), lean=bool(getattr(self, "lean_outputs", False)))
-        keep = (lambda t: t) if getattr(self, "static_outputs", False) else (lambda t: t.clone())
+        static = getattr(self, "static_outputs", False)
+        keep = (lambda t: t) if static else (lambda t: None if t is None else t.clone())   # None: lean_outputs
         H, W = eng.geo
-        gh, gw = H // PATCH, W // PATCH
-        N = gh * gw
         kps, depth, scr, dsc = keep(st["kps"]), keep(st["depth"]), keep(st["scr"]), keep(st["dsc"])
-        data["kps0_shape"], data["kps1_shape"], data["down_factor"] = [gh, gw], [gh, gw], self.compute_matches.down_factor
-        data["depth0_map"], data["depth1_map"] = depth[:B].reshape(B, 1, gh, gw), depth[B:].reshape(B, 1, gh, gw)
-        data["kps0"], data["kps1"] = kps[:B], kps[B:]
-        data["depth_kp0"], data["depth_kp1"] = depth[:B], depth[B:]
-        data["scr0"], data["scr1"] = scr[:B], scr[B:]
-        data["dsc0"], data["dsc1"] = dsc[:B], dsc[B:]
-        if st["scores"] is not None:             # lean_outputs: only final_scores (what the solver reads) is materialised
-            data["scores"], data["kp_scores"] = keep(st["scores"]), keep(st["kp_scores"])
+        _set_correspondences(data, kps, depth, (scr[:B], scr[B:]), (dsc[:B], dsc[B:]), (H // PATCH, W // PATCH),
+                             self.compute_matches.down_factor, keep(st["scores"]), keep(st["kp_scores"]))
         data["final_scores"] = keep(st["final_scores"])
-        pose = keep(st["pose"])
-        R, t, inliers = pose[:, :9].reshape(B, 3, 3), pose[:, 9:12].reshape(B, 1, 3), pose[:, 12:13]
+        R, t, inliers = _pose_views(keep(st["pose"]))
         if return_inliers:
-            data["inliers_list"] = self._inlier_list(data, st, B, N)
-        if not getattr(self, "static_outputs", False):
+            data["inliers_list"] = _inlier_list(st, data["final_scores"], data["kps0"], data["kps1"], data["depth_kp0"],
+                                                data["depth_kp1"])
+        if not static:
             eng.release()                                # every read of the static buffers above is queued
         data["R"], data["t"], data["inliers"] = R, t, inliers
         return R, t
@@ -461,20 +445,16 @@ class MickeyRelativePose(nn.Module):
         bank1 = tuple(t.float().contiguous() for t in feats1.tensors())
         st = eng.forward_pairs(bank0, t0, bank1, t1, K0.float(), K1.float(), seed, feats0.image_size,
                                lean=bool(getattr(self, "lean_outputs", False)))
-        gh, gw = feats0.grid
-        kps, depth = st["kps"], st["depth"]
-        data = {"kps0_shape": [gh, gw], "kps1_shape": [gh, gw], "down_factor": self.compute_matches.down_factor,
-                "depth0_map": depth[:P].reshape(P, 1, gh, gw), "depth1_map": depth[P:].reshape(P, 1, gh, gw),
-                "kps0": kps[:P], "kps1": kps[P:], "depth_kp0": depth[:P], "depth_kp1": depth[P:],
-                "scr0": bank0[2].index_select(0, t0.long()), "scr1": bank1[2].index_select(0, t1.long()),
-                "dsc0": bank0[3].index_select(0, t0.long()), "dsc1": bank1[3].index_select(0, t1.long())}
-        if st["scores"] is not None:
-            data["scores"], data["kp_scores"] = st["scores"], st["kp_scores"]
+        data = {}
+        _set_correspondences(data, st["kps"], st["depth"],
+                             (bank0[2].index_select(0, t0.long()), bank1[2].index_select(0, t1.long())),
+                             (bank0[3].index_select(0, t0.long()), bank1[3].index_select(0, t1.long())),
+                             feats0.grid, self.compute_matches.down_factor, st["scores"], st["kp_scores"])
         data["final_scores"] = st["final_scores"]
-        pose = st["pose"]
-        data["R"], data["t"], data["inliers"] = pose[:, :9].reshape(P, 3, 3), pose[:, 9:12].reshape(P, 1, 3), pose[:, 12:13]
+        data["R"], data["t"], data["inliers"] = _pose_views(st["pose"])
         if return_inliers:
-            data["inliers_list"] = self._inlier_list(data, st, P, gh * gw)
+            data["inliers_list"] = _inlier_list(st, data["final_scores"], data["kps0"], data["kps1"], data["depth_kp0"],
+                                                data["depth_kp1"])
         return data
 
     @torch.no_grad()
