@@ -142,6 +142,30 @@ int mk_solve_pose(mk_handle* h, const float* final_scores_dev, long long nn_pitc
                   float* inlier_mask_dev, int* sampled_idx_out_dev, float* hyp_scores_out_dev, int* status_dev,
                   void* ws_dev, long long ws_bytes, void* stream);
 
+/* ---- stage 3 without a handle: the same solver for callers that have no finalized handle, e.g. the training model's
+ * validation (mickey_b200/procrustes.py wraps it as a drop-in e2eProbabilisticProcrustesSolver).  Arguments, outputs and
+ * the status bits are those of mk_solve_pose, with N and every PROCRUSTES value given by the caller: it_matches /
+ * it_ransac / num_sampled / num_corr / num_refine / th_inlier / th_soft_inlier are IT_MATCHES / IT_RANSAC /
+ * NUM_SAMPLED_MATCHES / NUM_CORR_3D_3D / NUM_REFINEMENTS / TH_INLIER / TH_SOFT_INLIER.  kps_dev [2B,2,N], depth_dev
+ * [2B,1,N] (image-0 rows first), K0/K1 fp32 [B,3,3].  The seed is written into the workspace: there is no state across
+ * calls, and a call with seed s draws what mk_solve_pose draws after being reseeded with s (so, with the handle's
+ * PROCRUSTES values, every output is the same bits).
+ * Sizes, from the kernels: 1 <= B <= 65535 and 1 <= it_matches <= 65535 (grid dimensions), N >= 1 with N*N < 2^31 (int32
+ * cell indices), it_ransac >= 1 with it_matches*it_ransac < 2^31 and B*it_matches < 2^31, num_sampled a multiple of 256
+ * (the hypothesis kernel scans a set across 256 threads) up to 2048 (the sampler's selection sorts 2048 candidates),
+ * num_corr = 3 (the inner draw and the hypotheses' Kabsch take three correspondences), num_refine >= 0, both thresholds
+ * finite and positive.  The shipped configurations use 2048 / 3 / 4.
+ * Workspace: mk_procrustes_ws_bytes(B, N, it_matches, it_ransac, num_sampled) bytes, 256-byte aligned (-1 for
+ * unsupported sizes).  Bad arguments (a NULL input, pose or workspace, an unsupported size, nn_pitch < N, a small
+ * workspace) return MK_ERR_INVALID with a message and launch nothing. */
+long long mk_procrustes_ws_bytes(int B, int N, int it_matches, int it_ransac, int num_sampled);
+int mk_procrustes_solve(const float* final_scores_dev, long long nn_pitch, const float* kps_dev, const float* depth_dev,
+                        const float* K0_dev, const float* K1_dev, int B, int N, int it_matches, int it_ransac,
+                        int num_sampled, int num_corr, int num_refine, float th_inlier, float th_soft_inlier,
+                        unsigned long long seed, const int* outer_idx_dev, const int* inner_idx_dev, float* pose_dev,
+                        int* best_set_dev, float* inlier_mask_dev, int* sampled_idx_out_dev, float* hyp_scores_out_dev,
+                        int* status_dev, void* ws_dev, long long ws_bytes, void* stream);
+
 /* ---- whole path: replaces MickeyRelativePose.forward (compute_pose.py:20-37) ---- */
 int mk_forward(mk_handle* h, const float* images_dev, const float* K0_dev, const float* K1_dev, int n_pairs,
                int img_h, int img_w, unsigned long long seed, float* kps_dev, float* depth_dev, float* scr_dev,

@@ -5,6 +5,7 @@
 #include "ops.h"
 
 #include <algorithm>
+#include <cfloat>
 #include <cstring>
 #include <string>
 #include <unordered_map>
@@ -61,6 +62,21 @@ struct Carver {
   }
 };
 
+// The solver's scratch: the sampler's histogram and candidates, the drawn cells, every hypothesis's score and [R | t],
+// the status word with the fused kernel's completion counters, and the winning hypothesis of each pair.
+struct SolverWs { void* samp_ws; int* idx; float* hyp_scores; float* hyp_Rt; int* status; int* best_hyp; };
+
+// Carved last in the handle's workspace (mk_solve_pose, mk_forward*) and alone in mk_procrustes_solve's.
+void carve_solver(Carver& cv, int n_pairs, int it_matches, int it_ransac, int num_sampled, SolverWs& s) {
+  const size_t streams = (size_t)n_pairs * it_matches;
+  s.samp_ws = cv.take<uint8_t>(sampler_workspace_bytes(n_pairs, it_matches));
+  s.idx = cv.take<int>(streams * num_sampled);
+  s.hyp_scores = cv.take<float>(streams * it_ransac);
+  s.hyp_Rt = cv.take<float>(streams * it_ransac * 12);
+  s.status = cv.take<int>(SOLVER_COUNTER_BASE + n_pairs);     // status bits + the fused solver's completion counters
+  s.best_hyp = cv.take<int>(n_pairs);
+}
+
 struct Workspace {
   // backbone
   __half* P; float* X; __half* XN; __half* QKV; __half* ATT; __half* H1;
@@ -71,8 +87,7 @@ struct Workspace {
   float* score_raw; __half* DSCX; float* nrm2; float* scr_copy;
   // matcher
   float *part_row, *part_col, *lse_r, *lse_c;
-  // solver
-  void* samp_ws; int* idx; float* hyp_scores; float* hyp_Rt; int* status; int* best_hyp;
+  SolverWs sol;
   size_t bytes;
 };
 
@@ -121,13 +136,7 @@ Workspace carve(void* base, const mk_config& c, const Geo& g) {
   const size_t npad = (size_t)ceil_div(g.N, 128) * 128;          // matcher: float2 partials [pair][slot][npad], lse vectors [pair][npad]
   w.part_row = cv.take<float>((size_t)n_pairs * (npad / 64) * npad * 2); w.part_col = cv.take<float>((size_t)n_pairs * (npad / 32) * npad * 2);
   w.lse_r = cv.take<float>((size_t)n_pairs * npad); w.lse_c = cv.take<float>((size_t)n_pairs * npad);
-  const size_t streams = (size_t)n_pairs * c.it_matches;
-  w.samp_ws = cv.take<uint8_t>(sampler_workspace_bytes(n_pairs, c.it_matches));
-  w.idx = cv.take<int>(streams * c.num_sampled);
-  w.hyp_scores = cv.take<float>(streams * c.it_ransac);
-  w.hyp_Rt = cv.take<float>(streams * c.it_ransac * 12);
-  w.status = cv.take<int>(SOLVER_COUNTER_BASE + n_pairs);     // status bits + the fused solver's completion counters
-  w.best_hyp = cv.take<int>(n_pairs);
+  carve_solver(cv, n_pairs, c.it_matches, c.it_ransac, c.num_sampled, w.sol);
   w.bytes = cv.off + 256;
   return w;
 }
@@ -168,10 +177,11 @@ void set_conv_taps(GemmParams& p, int cin, int w2, bool three) {
   p.k_chunks = p.num_taps * p.chunks_per_tap;
 }
 
+// h == NULL (the handle-free solver) records nothing
 struct ProfScope {
   mk_handle* h; cudaStream_t st; int slot = -1;
   ProfScope(mk_handle* h_, const char* tag, cudaStream_t st_) : h(h_), st(st_) {
-    if (!h->profiling) return;
+    if (!h || !h->profiling) return;
     mk_handle::ProfRec r;
     r.tag = tag;
     if (cudaEventCreate(&r.e0) != cudaSuccess || cudaEventCreate(&r.e1) != cudaSuccess) return;
@@ -410,37 +420,71 @@ int run_match(mk_handle* h, int n_pairs, int N, float* scores, float* kp_scores,
 }
 
 // ---- stage 3 ----------------------------------------------------------------------------------------------
-int run_solve(mk_handle* h, const float* final_scores, long long nn_pitch, const float* kps, const float* depth, const float* K0,
-              const float* K1, int n_pairs, int N, unsigned long long seed, const int* outer_idx, const int* inner_idx,
-              float* pose, int* best_set, float* inl_mask, int* sampled_out, float* hyp_scores_out, int* status_out,
-              Workspace& w, cudaStream_t st) {
-  const mk_config& c = h->cfg;
-  RansacParams rp{c.it_matches, c.it_ransac, c.num_sampled, c.num_corr, c.num_refine, c.th_inlier, c.th_soft_inlier, h->seed_dev};
-  MK_TRY(resolve_pitch(nn_pitch, N, "mk_solve_pose: nn_pitch"));
-  if (seed != 0) MK_TRY(seed_set(h->seed_dev, seed, st));      // seed == 0: continue the device-side sequence
-  MK_CUDA_CHECK(cudaMemsetAsync(w.status, 0, (size_t)(SOLVER_COUNTER_BASE + n_pairs) * sizeof(int), st));
-  const size_t n_idx = (size_t)n_pairs * c.it_matches * c.num_sampled;
+// The solve of one batch: the outer draw (unless outer_idx is given), the fused RANSAC kernel and the optional output
+// copies, in the solver's scratch s.  rp holds the PROCRUSTES sizes and rp.seed the device word both draws read; nn_pitch
+// is resolved.  h: the handle of mk_solve_pose / mk_forward*, whose profiling scopes and launch count this feeds, or NULL
+// (mk_procrustes_solve).
+int run_solve(mk_handle* h, const RansacParams& rp, const float* final_scores, long long nn_pitch, const float* kps,
+              const float* depth, const float* K0, const float* K1, int n_pairs, int N, const int* outer_idx,
+              const int* inner_idx, float* pose, int* best_set, float* inl_mask, int* sampled_out, float* hyp_scores_out,
+              int* status_out, const SolverWs& s, cudaStream_t st) {
+  MK_CUDA_CHECK(cudaMemsetAsync(s.status, 0, (size_t)(SOLVER_COUNTER_BASE + n_pairs) * sizeof(int), st));
+  const size_t n_idx = (size_t)n_pairs * rp.it_matches * rp.n_sample;
   const int* idx = outer_idx;
   if (!idx) {
-    { ProfScope ps_(h, "solve.sample_outer", st); h->launches += 4;
-      MK_TRY(sample_outer(final_scores, n_pairs, N, nn_pitch, c.it_matches, c.num_sampled, h->seed_dev, w.samp_ws, w.idx, w.status, st)); }
-    idx = w.idx;
+    { ProfScope ps_(h, "solve.sample_outer", st); if (h) h->launches += 4;
+      MK_TRY(sample_outer(final_scores, n_pairs, N, nn_pitch, rp.it_matches, rp.n_sample, rp.seed, s.samp_ws, s.idx, s.status, st)); }
+    idx = s.idx;
   }
   const float* kps0 = kps;
   const float* kps1 = kps + (size_t)n_pairs * 2 * N;
   const float* d0 = depth;
   const float* d1 = depth + (size_t)n_pairs * N;
-  int* bs = best_set ? best_set : w.best_hyp;     // scratch when the caller does not want it
-  { ProfScope ps_(h, "solve.ransac", st); h->launches += 1;
-    MK_TRY(ransac_solve(final_scores, nn_pitch, kps0, d0, kps1, d1, K0, K1, n_pairs, N, rp, idx, inner_idx, w.hyp_scores,
-                        w.hyp_Rt, w.status, pose, bs, inl_mask, best_set ? w.best_hyp : nullptr, st)); }
-  MK_TRY(seed_advance(h->seed_dev, st));
+  int* bs = best_set ? best_set : s.best_hyp;     // scratch when the caller does not want it
+  { ProfScope ps_(h, "solve.ransac", st); if (h) h->launches += 1;
+    MK_TRY(ransac_solve(final_scores, nn_pitch, kps0, d0, kps1, d1, K0, K1, n_pairs, N, rp, idx, inner_idx, s.hyp_scores,
+                        s.hyp_Rt, s.status, pose, bs, inl_mask, best_set ? s.best_hyp : nullptr, st)); }
   if (sampled_out) MK_CUDA_CHECK(cudaMemcpyAsync(sampled_out, idx, n_idx * sizeof(int), cudaMemcpyDeviceToDevice, st));
   if (hyp_scores_out)
-    MK_CUDA_CHECK(cudaMemcpyAsync(hyp_scores_out, w.hyp_scores, (size_t)n_pairs * c.it_matches * c.it_ransac * sizeof(float),
+    MK_CUDA_CHECK(cudaMemcpyAsync(hyp_scores_out, s.hyp_scores, (size_t)n_pairs * rp.it_matches * rp.it_ransac * sizeof(float),
                                   cudaMemcpyDeviceToDevice, st));
-  if (status_out) MK_CUDA_CHECK(cudaMemcpyAsync(status_out, w.status, sizeof(int), cudaMemcpyDeviceToDevice, st));
+  if (status_out) MK_CUDA_CHECK(cudaMemcpyAsync(status_out, s.status, sizeof(int), cudaMemcpyDeviceToDevice, st));
   return MK_OK;
+}
+
+// The handle's solve: its PROCRUSTES config and its device-side seed, which a non-zero seed resets and every solve advances.
+int run_solve_handle(mk_handle* h, const float* final_scores, long long nn_pitch, const float* kps, const float* depth,
+                     const float* K0, const float* K1, int n_pairs, int N, unsigned long long seed, const int* outer_idx,
+                     const int* inner_idx, float* pose, int* best_set, float* inl_mask, int* sampled_out,
+                     float* hyp_scores_out, int* status_out, Workspace& w, cudaStream_t st) {
+  const mk_config& c = h->cfg;
+  RansacParams rp{c.it_matches, c.it_ransac, c.num_sampled, c.num_corr, c.num_refine, c.th_inlier, c.th_soft_inlier, h->seed_dev};
+  MK_TRY(resolve_pitch(nn_pitch, N, "mk_solve_pose: nn_pitch"));
+  if (seed != 0) MK_TRY(seed_set(h->seed_dev, seed, st));      // seed == 0: continue the device-side sequence
+  MK_TRY(run_solve(h, rp, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, N, outer_idx, inner_idx, pose, best_set,
+                   inl_mask, sampled_out, hyp_scores_out, status_out, w.sol, st));
+  return seed_advance(h->seed_dev, st);
+}
+
+// mk_procrustes_solve's sizes (include/mickey_b200.h): the sampler's selection sorts 2048 candidates per stream and the
+// hypothesis kernel scans a set across its 256 threads; one grid dimension holds B, another IT_MATCHES; cells, hypotheses
+// of a pair and streams are counted in int.
+constexpr int PROC_MAX_SAMPLED = 2048, PROC_SAMPLED_STEP = 256, PROC_MAX_GRID = 65535;
+
+bool procrustes_sizes_ok(int B, int N, int it_matches, int it_ransac, int num_sampled) {
+  return B >= 1 && B <= PROC_MAX_GRID && N >= 1 && (long long)N * N <= 0x7fffffffLL && it_matches >= 1 &&
+         it_matches <= PROC_MAX_GRID && it_ransac >= 1 && (long long)it_matches * it_ransac <= 0x7fffffffLL &&
+         (long long)B * it_matches <= 0x7fffffffLL && num_sampled >= PROC_SAMPLED_STEP && num_sampled <= PROC_MAX_SAMPLED &&
+         num_sampled % PROC_SAMPLED_STEP == 0;
+}
+
+// the solver's scratch, then the seed word
+size_t procrustes_carve(void* ws, int B, int it_matches, int it_ransac, int num_sampled, SolverWs& s,
+                        unsigned long long** seed_word) {
+  Carver cv(ws);
+  carve_solver(cv, B, it_matches, it_ransac, num_sampled, s);
+  *seed_word = cv.take<unsigned long long>(1);
+  return (cv.off + 255) & ~(size_t)255;
 }
 
 int check_ws(mk_handle* h, int n_img, int n_pairs, int H, int W, void* ws, long long ws_bytes, Workspace& out) {
@@ -627,8 +671,50 @@ int mk_solve_pose(mk_handle* h, const float* final_scores, long long nn_pitch, c
   MK_TRY(check_ws(h, 2 * n_pairs, n_pairs, h ? h->geo_h : 0, h ? h->geo_w : 0, ws, ws_bytes, w));
   const Geo g = make_geo(2 * n_pairs, n_pairs, h->geo_h, h->geo_w);
   if (n_kpts != g.N) { set_last_error("n_kpts %d does not match the geometry (%d)", n_kpts, g.N); return MK_ERR_INVALID; }
-  return run_solve(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, n_kpts, seed, outer_idx, inner_idx, pose, best_set,
-                   inl_mask, sampled_out, hyp_scores_out, status, w, (cudaStream_t)stream);
+  return run_solve_handle(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, n_kpts, seed, outer_idx, inner_idx, pose,
+                          best_set, inl_mask, sampled_out, hyp_scores_out, status, w, (cudaStream_t)stream);
+}
+
+long long mk_procrustes_ws_bytes(int B, int N, int it_matches, int it_ransac, int num_sampled) {
+  if (!procrustes_sizes_ok(B, N, it_matches, it_ransac, num_sampled)) return -1;
+  SolverWs s;
+  unsigned long long* seed_word;
+  return (long long)procrustes_carve(nullptr, B, it_matches, it_ransac, num_sampled, s, &seed_word);
+}
+
+int mk_procrustes_solve(const float* final_scores, long long nn_pitch, const float* kps, const float* depth, const float* K0,
+                        const float* K1, int B, int N, int it_matches, int it_ransac, int num_sampled, int num_corr,
+                        int num_refine, float th_inlier, float th_soft_inlier, unsigned long long seed, const int* outer_idx,
+                        const int* inner_idx, float* pose, int* best_set, float* inl_mask, int* sampled_out,
+                        float* hyp_scores_out, int* status, void* ws, long long ws_bytes, void* stream) {
+  // every argument is checked before anything is launched
+  if (!final_scores || !kps || !depth || !K0 || !K1 || !pose || !ws) {
+    set_last_error("mk_procrustes_solve: final_scores, kps, depth, K0, K1, pose and the workspace must be non-NULL");
+    return MK_ERR_INVALID;
+  }
+  if (!procrustes_sizes_ok(B, N, it_matches, it_ransac, num_sampled) || num_corr != 3 || num_refine < 0 ||
+      !(th_inlier > 0.f && th_inlier <= FLT_MAX) || !(th_soft_inlier > 0.f && th_soft_inlier <= FLT_MAX)) {
+    set_last_error("mk_procrustes_solve: need 1 <= B <= %d, N >= 1 with N*N < 2^31, 1 <= it_matches <= %d, it_ransac >= 1, "
+                   "it_matches*it_ransac and B*it_matches < 2^31, num_sampled a multiple of %d up to %d, num_corr 3, "
+                   "num_refine >= 0 and finite positive thresholds (got B %d N %d it_matches %d it_ransac %d num_sampled %d "
+                   "num_corr %d num_refine %d th_inlier %g th_soft_inlier %g)", PROC_MAX_GRID, PROC_MAX_GRID,
+                   PROC_SAMPLED_STEP, PROC_MAX_SAMPLED, B, N, it_matches, it_ransac, num_sampled, num_corr, num_refine,
+                   (double)th_inlier, (double)th_soft_inlier);
+    return MK_ERR_INVALID;
+  }
+  MK_TRY(resolve_pitch(nn_pitch, N, "mk_procrustes_solve: nn_pitch"));
+  SolverWs s;
+  unsigned long long* seed_word;
+  const size_t need = procrustes_carve(ws, B, it_matches, it_ransac, num_sampled, s, &seed_word);
+  if ((long long)need > ws_bytes) {
+    set_last_error("mk_procrustes_solve: workspace of %lld bytes, %zu needed", ws_bytes, need);
+    return MK_ERR_INVALID;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const RansacParams rp{it_matches, it_ransac, num_sampled, num_corr, num_refine, th_inlier, th_soft_inlier, seed_word};
+  MK_TRY(seed_set(seed_word, seed, st));
+  return run_solve(nullptr, rp, final_scores, nn_pitch, kps, depth, K0, K1, B, N, outer_idx, inner_idx, pose, best_set,
+                   inl_mask, sampled_out, hyp_scores_out, status, s, st);
 }
 
 static int forward_any(mk_handle* h, const void* images, int img_fmt, const float* K0, const float* K1, int n_pairs, int H, int W,
@@ -641,8 +727,8 @@ static int forward_any(mk_handle* h, const void* images, int img_fmt, const floa
   cudaStream_t st = (cudaStream_t)stream;
   MK_TRY(run_extract(h, images, img_fmt, g, kps, depth, scr, dsc, w, st));
   MK_TRY(run_match(h, n_pairs, g.N, scores, kp_scores, final_scores, nn_pitch, w, st));
-  return run_solve(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, g.N, seed, nullptr, nullptr, pose, best_set, inl_mask,
-                   sampled_out, nullptr, status, w, st);
+  return run_solve_handle(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, g.N, seed, nullptr, nullptr, pose, best_set,
+                          inl_mask, sampled_out, nullptr, status, w, st);
 }
 
 int mk_forward(mk_handle* h, const float* images, const float* K0, const float* K1, int n_pairs, int H, int W,
@@ -679,8 +765,8 @@ int mk_forward_pairs(mk_handle* h, const float* kps0, const float* depth0, const
   const BankView b0{kps0, depth0, scr0, dsc0, idx0, n0}, b1{kps1, depth1, scr1, dsc1, idx1, n1};
   MK_KERNEL("pairs.gather", bank_gather(b0, b1, n_pairs, g.N, w.DSCX, kps, depth, w.scr_copy, st));
   MK_TRY(run_match(h, n_pairs, g.N, scores, kp_scores, final_scores, nn_pitch, w, st));
-  MK_TRY(run_solve(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, g.N, seed, nullptr, nullptr, pose, best_set, inl_mask,
-                   sampled_out, nullptr, status, w, st));
+  MK_TRY(run_solve_handle(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, g.N, seed, nullptr, nullptr, pose, best_set,
+                          inl_mask, sampled_out, nullptr, status, w, st));
   MK_KERNEL("pairs.index_check", bank_index_check(b0, b1, n_pairs, pose, status, st));
   return MK_OK;
 }
@@ -732,8 +818,8 @@ long long mk_workspace_offset(mk_handle* h, const char* name, int n_pairs, int H
       {"S1", w.S1}, {"O1", w.O1}, {"T2", w.T2}, {"S2", w.S2}, {"O2", w.O2}, {"T3", w.T3}, {"S3", w.S3}, {"CAT", w.CAT},
       {"MSG", w.MSG}, {"HM", w.HM}, {"T4k", w.T4k}, {"S4k", w.S4k}, {"T4d", w.T4d}, {"X32", w.X32}, {"QKV32", w.QKV32},
       {"KV", w.KV}, {"Y4k", w.Y4k}, {"Y4d", w.Y4d}, {"score_raw", w.score_raw}, {"DSCX", w.DSCX}, {"nrm2", w.nrm2},
-      {"lse_r", w.lse_r}, {"lse_c", w.lse_c}, {"idx", w.idx}, {"hyp_scores", w.hyp_scores},
-      {"hyp_Rt", w.hyp_Rt}};
+      {"lse_r", w.lse_r}, {"lse_c", w.lse_c}, {"idx", w.sol.idx}, {"hyp_scores", w.sol.hyp_scores},
+      {"hyp_Rt", w.sol.hyp_Rt}};
   auto it = m.find(name);
   if (it == m.end()) { set_last_error("unknown workspace buffer '%s'", name); return -1; }
   return (long long)(reinterpret_cast<const uint8_t*>(it->second) - base);

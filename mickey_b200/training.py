@@ -4,6 +4,7 @@
 
     model = MicKeyTrainingModel(cfg)
     use_cuda_modules(model)            # before trainer.fit, so that configure_optimizers collects the new modules' Parameters
+    use_cuda_modules(model, solver=True)   # the same, and the validation's pose solver too
     trainer.fit(model, datamodule)
 
 See use_cuda_modules for what moves and what is kept.
@@ -18,6 +19,7 @@ from .dinov2 import DinoVisionTransformer
 from .dual_softmax import dualSoftmax
 from .heads import DeepResBlock_depth, DeepResBlock_desc, DeepResBlock_det, DeepResBlock_offset
 from .loss import MetricPoseLoss
+from .procrustes import e2eProbabilisticProcrustesSolver
 
 HEADS = {"depth_head": DeepResBlock_depth, "det_offset": DeepResBlock_offset, "dsc_head": DeepResBlock_desc,
          "det_head": DeepResBlock_det}
@@ -53,7 +55,7 @@ def _transplant(new: nn.Module, old: nn.Module):
         m.training = flags.setdefault(n, flags[n.rpartition(".")[0]])
 
 
-def use_cuda_modules(model):
+def use_cuda_modules(model, solver: bool = False):
     """Replace, in place, the modules of the reference's MicKeyTrainingModel that have CUDA drop-ins, and return model:
 
         compute_matches.extractor.dinov2_vitl14      -> mickey_b200.dinov2.DinoVisionTransformer (the variant of its width)
@@ -61,12 +63,15 @@ def use_cuda_modules(model):
                                                      -> mickey_b200.heads.DeepResBlock_{det, offset, depth, desc}
         compute_matches.matcher.matching_mat         -> mickey_b200.dual_softmax.dualSoftmax
         loss_fn                                      -> mickey_b200.loss.MetricPoseLoss
+        e2e_Procrustes (with solver=True)            -> mickey_b200.procrustes.e2eProbabilisticProcrustesSolver
 
     Each new module takes over the old one's Parameter and buffer objects, so model.state_dict() keeps its keys, shapes,
     dtypes and values bit for bit (BN running statistics, num_batches_tracked and an fp16 backbone under DINOV2.FLOAT16
     included), as do every requires_grad, every module's training flag and every device.  The loss keeps its topK, the
     curriculum state on_train_epoch_end moves, when the reference's loss has one (only with top-K or curriculum training).
-    DINOV2.FLOAT16: False is rejected: the CUDA backbone runs in fp16 only.  model.e2e_Procrustes (validation and logging) stays the reference's.
+    DINOV2.FLOAT16: False is rejected: the CUDA backbone runs in fp16 only.  model.e2e_Procrustes, the pose solver of the
+    validation step and of the logging in backward_step, is replaced only with solver=True (it holds no parameters or
+    buffers, so the state dict is the same either way); by default it stays the reference's.
 
     Call it before trainer.fit, so that configure_optimizers collects the new modules' Parameters.  Every replacement is
     built and checked before the model is touched: a configuration a drop-in rejects raises ValueError and leaves the
@@ -106,10 +111,15 @@ def use_cuda_modules(model):
         if hasattr(old, "topK"):                 # the reference sets it only with top-K or curriculum training
             new.topK = old.topK
         swaps.append((model, "loss_fn", new, old))
+    procrustes = None
+    if solver and not isinstance(getattr(model, "e2e_Procrustes", None), e2eProbabilisticProcrustesSolver):
+        procrustes = e2eProbabilisticProcrustesSolver(cfg)
 
     for parent, name, new, old in swaps:
         _check_trees(new, old, name)
     for parent, name, new, old in swaps:
         _transplant(new, old)
         setattr(parent, name, new)
+    if procrustes is not None:
+        model.e2e_Procrustes = procrustes
     return model
