@@ -166,6 +166,26 @@ int mk_procrustes_solve(const float* final_scores_dev, long long nn_pitch, const
                         int* best_set_dev, float* inlier_mask_dev, int* sampled_idx_out_dev, float* hyp_scores_out_dev,
                         int* status_dev, void* ws_dev, long long ws_bytes, void* stream);
 
+/* ---- grading a Map-free submission: the per-frame errors of the benchmark's MetricManager (benchmark/metrics.py:
+ * trans_err, rot_err with the sin variant, reproj_err), fp64.  mickey_b200/mapfree_eval.py restates the benchmark's host
+ * logic around it.  No handle, no workspace, no state between calls; enqueued on `stream`.  For P frames, row-major
+ * device arrays:
+ *   q_est_dev [P,4], t_est_dev [P,3]: each estimate as its submission line holds it (world-to-camera, qw qx qy qz tx ty tz);
+ *   q_gt_dev [P,4], t_gt_dev [P,3]:   the ground truth of poses.txt, in the same convention;
+ *   K_dev [P,3,3]:                    each frame's intrinsics;
+ *   grid_dev [MK_VCRE_POINTS,3]:      the virtual points, mickey_b200.loss.vcre_grid();
+ *   W, H:                             the image size both projections are clipped to (shared by the call's frames).
+ * A quaternion need not be unit: as in the benchmark, its norm scales the camera centre (by 1/|q|^4) but not the rotation.
+ * Out: err_dev fp64 [P,3] = trans_err (m), rot_err (deg), reproj_err (px); csrc/mapfree_eval.cu states each formula.
+ * A frame's values are the same bits alone, inside any batch and on every run.
+ * Bad arguments (a NULL pointer, P < 1 or P > MK_MAPFREE_MAX_FRAMES, W < 1 or H < 1) return MK_ERR_INVALID with a
+ * message and launch nothing. */
+#define MK_VCRE_POINTS 196
+#define MK_MAPFREE_MAX_FRAMES 67108863   /* one warp per frame: 32 * P threads index in int32 */
+int mk_mapfree_frame_metrics(const double* q_est_dev, const double* t_est_dev, const double* q_gt_dev,
+                             const double* t_gt_dev, const double* K_dev, const double* grid_dev, int P, int W, int H,
+                             double* err_dev, void* stream);
+
 /* ---- whole path: replaces MickeyRelativePose.forward (compute_pose.py:20-37) ---- */
 int mk_forward(mk_handle* h, const float* images_dev, const float* K0_dev, const float* K1_dev, int n_pairs,
                int img_h, int img_w, unsigned long long seed, float* kps_dev, float* depth_dev, float* scr_dev,

@@ -9,8 +9,9 @@ list, takes its contiguous slice (lib/datasets/sampler.py), runs the CUDA hot pa
 all-gather of the packed [batch, 13] poses per step (ranks whose slice is exhausted contribute an empty block).  Rank 0
 converts the gathered poses to submission records on its GPU (mk_pose_to_submission, one D2H per step), writes
 `submission.zip` with the reference's `pose_<scene>.txt` line format, and grades the poses against the tree's ground
-truth with the reference's pose-error definitions (lib/utils/metrics.py:12-53).  With random-init weights the poses
-are noise — the run proves the plumbing and gives pairs/s end to end from JPEG files.
+truth with the reference's pose-error definitions (lib/utils/metrics.py:12-53).  `--evaluate` also grades the written zip
+as the Map-free benchmark does (mickey_b200/mapfree_eval.py) and adds its numbers under "mapfree_metrics".  With
+random-init weights the poses are noise — the run proves the plumbing and gives pairs/s end to end from JPEG files.
 
 Every val/test pair of a scene has the same image0, the scene's reference image.  `--share-reference` reads and extracts
 each reference once (ReferenceBank), extracts only the query images of a step and poses the batch from the two feature
@@ -84,6 +85,8 @@ def main():
     ap.add_argument("--seed", type=int, default=None,
                     help="seed the torch RNG that the solver's per-batch seeds come from (a reproducible submission)")
     ap.add_argument("--output_root", "-o", type=Path, default=Path("results/"))
+    ap.add_argument("--evaluate", action="store_true",
+                    help="grade the written submission.zip as the Map-free benchmark does (summary key mapfree_metrics)")
     args = ap.parse_args()
 
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
@@ -190,6 +193,10 @@ def main():
             r_err, t_err = pose_errors(Rm, recs[ok, 4:7], np.stack(T_gt)[ok].astype(np.float64))
             summary.update(median_R_err_deg=float(np.median(r_err)) if ok.any() else None,
                            median_t_err_m=float(np.median(t_err)) if ok.any() else None)
+        if args.evaluate:
+            from mickey_b200.mapfree_eval import evaluate_submission
+            summary["mapfree_metrics"], _ = evaluate_submission(cfg.DATASET.DATA_ROOT, args.output_root / "submission.zip",
+                                                                args.split)
         print(json.dumps(summary), flush=True)
     if world > 1:
         import torch.distributed as dist
