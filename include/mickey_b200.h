@@ -301,7 +301,7 @@ long long mk_loss_gradient_ws_bytes(int B, int it_matches, int n_sample);
  *
  * Workspaces: mk_dual_softmax_ws_bytes(B, N) / mk_dual_softmax_backward_ws_bytes(B, N) bytes, 256-byte aligned (0 for
  * unsupported sizes).  Bad arguments return MK_ERR_INVALID and launch nothing.  Both calls always use the wgmma and
- * fp32 kernels; MICKEY_GEMM_IMPL does not apply to them.  Capturing them in a CUDA graph is not tested. */
+ * fp32 kernels.  Capturing them in a CUDA graph is not tested. */
 long long mk_dual_softmax_ws_bytes(int B, int N);
 long long mk_dual_softmax_backward_ws_bytes(int B, int N);
 int mk_dual_softmax(const float* dsc0_dev, const float* dsc1_dev, const float* scr0_dev, const float* scr1_dev,
@@ -462,8 +462,7 @@ int mk_profile_read(mk_handle* h, char* buf, int buf_bytes);
 
 /* ---- operator-level entry points (unit tests of single kernels; not needed by an integrator) ---- */
 typedef struct mk_gemm_args {
-  int epi;                 /* 0 STORE_H, 1 RESID_F, 2 PATCH, 3 CONV, 4 STORE_F, 5 LN, 6 LSE (row + column partials), 7 DUAL,
-                              8 RESID_LN (RESID_F, then out_h = LayerNorm(out_f row) * aux + beta; N <= 1024) */
+  int epi;                 /* 0 STORE_H, 1 RESID_F, 2 PATCH, 3 CONV, 4 STORE_F, 5 LN, 6 LSE (row + column partials), 7 DUAL */
   int impl;                /* 0 default (wgmma), 1 wgmma, 2 SIMT debug kernel; 3 / 4: the persistent wgmma kernel with /
                               without two-CTA pairs sharing B, on any grid (the epilogues it does not serve run as 1) */
   const void* a; long long a_rows, a_cols, a_ld;

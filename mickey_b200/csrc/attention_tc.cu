@@ -20,8 +20,6 @@
 #include "ops.h"
 #include "gemm.h"
 #include <algorithm>
-#include <cstdlib>
-#include <cstring>
 
 namespace mk {
 
@@ -258,14 +256,9 @@ int attention_tc(const void* qkv, void* out, int n_img, int T, int D, int heads,
   return MK_OK;
 }
 
-// impl: 0 = default (wgmma unless MICKEY_ATTN_IMPL=mma), 1 = wgmma, 2 = mma.sync
+// impl: 0 = default (wgmma), 1 = wgmma, 2 = mma.sync
 int attention_dispatch(const void* qkv, void* out, int n_img, int T, int D, int heads, int impl, cudaStream_t s) {
-  if (impl == 0) {
-    static int def = 0;
-    if (!def) { const char* e = getenv("MICKEY_ATTN_IMPL"); def = (e && strcmp(e, "mma") == 0) ? 2 : 1; }
-    impl = def;
-  }
-  if (impl != 1 && impl != 2) { set_last_error("attention: unknown impl %d", impl); return MK_ERR_INVALID; }
+  if (impl < 0 || impl > 2) { set_last_error("attention: unknown impl %d", impl); return MK_ERR_INVALID; }
   return impl == 2 ? attention(qkv, out, n_img, T, D, heads, s) : attention_tc(qkv, out, n_img, T, D, heads, s);
 }
 

@@ -27,9 +27,6 @@ enum Epi : int {
   EPI_LN      = 5,   // out = LN_128(acc) [+ out_f]        fp16 (+fp32)   (merge+norm1, mlp.2+norm2+residual)
   EPI_LSE     = 6,   // per-tile (max, sum exp) partials of every row AND every column of S/T   (matcher pass 1)
   EPI_DUAL    = 7,   // scores = exp(2 S/T - lse_row - lse_col), kp_scores, final_scores          (matcher pass 2)
-  EPI_RESID_LN = 8,  // EPI_RESID_F, then out_h = LN_N(out_f row) * aux + beta   (attn.proj + norm2, mlp.fc2 + next norm1):
-                     // the N/128 CTAs of a row of tiles form a thread-block cluster and exchange row statistics
-                     // through distributed shared memory (N <= 1024)
 };
 
 enum Act : int { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2 };

@@ -222,7 +222,6 @@ int run_backbone(mk_handle* h, const void* images, int img_fmt, const Geo& g, Wo
     MK_TRY(gemm(h, "vit.patch_embed", EPI_PATCH, w.P, g.Mp, KPAD, wt, D, KPAD, p, st));
   }
   // -- transformer blocks (layers/block.py:105-106)
-  const bool fuse_ln = gemm_resid_ln_supported((int)g.M, D, D / 64) && gemm_resid_ln_supported((int)g.M, D, 4 * D / 64);
   for (int i = 0; i < c.depth; ++i) {
     const std::string b = "blk" + std::to_string(i) + ".";
     const float *ln1w = L.f(b + "ln1.w", D), *ln1b = L.f(b + "ln1.b", D), *ln2w = L.f(b + "ln2.w", D), *ln2b = L.f(b + "ln2.b", D);
@@ -231,27 +230,17 @@ int run_backbone(mk_handle* h, const void* images, int img_fmt, const Geo& g, Wo
     const float *bqkv = L.f(b + "qkv.b", 3 * D), *bproj = L.f(b + "proj.b", D), *bfc1 = L.f(b + "fc1.b", 4 * D), *bfc2 = L.f(b + "fc2.b", D);
     const float *ls1 = L.f(b + "ls1", D), *ls2 = L.f(b + "ls2", D);
     if (!L.ok) return MK_ERR_MISSING_TENSOR;
-    // LayerNorm rides in the epilogue of the GEMM that produces its input whenever that GEMM runs on a one-tile
-    // kernel (EPI_RESID_LN: cluster of N/128 CTAs, row statistics through DSMEM): norm2 in attn.proj, the next
-    // block's norm1 in mlp.fc2.  Only the first norm1 (after the patch embedding) and the final norm stay kernels.
-    if (i == 0 || !fuse_ln) MK_KERNEL("vit.layernorm", layernorm(w.X, ln1w, ln1b, w.XN, (int)g.M, D, 1e-6f, 0, 0, 0, st));
+    MK_KERNEL("vit.layernorm", layernorm(w.X, ln1w, ln1b, w.XN, (int)g.M, D, 1e-6f, 0, 0, 0, st));
     { GemmParams p = base_params(g.M, 3 * D, D); p.bias = bqkv; p.out_h = w.QKV; p.out_h_ld = 3 * D;
       MK_TRY(gemm(h, "vit.qkv", EPI_STORE_H, w.XN, g.M, D, wqkv, 3 * D, D, p, st)); }
     MK_KERNEL("vit.attention", attention_dispatch(w.QKV, w.ATT, g.n_img, g.T, D, c.heads, 0, st));
     { GemmParams p = base_params(g.M, D, D); p.bias = bproj; p.gamma = ls1; p.out_f = w.X; p.out_f_ld = D;
-      if (fuse_ln) { p.aux = ln2w; p.beta = ln2b; p.out_h = w.XN; p.out_h_ld = D; p.eps = 1e-6f; }
-      MK_TRY(gemm(h, "vit.proj", fuse_ln ? EPI_RESID_LN : EPI_RESID_F, w.ATT, g.M, D, wproj, D, D, p, st)); }
-    if (!fuse_ln) MK_KERNEL("vit.layernorm", layernorm(w.X, ln2w, ln2b, w.XN, (int)g.M, D, 1e-6f, 0, 0, 0, st));
+      MK_TRY(gemm(h, "vit.proj", EPI_RESID_F, w.ATT, g.M, D, wproj, D, D, p, st)); }
+    MK_KERNEL("vit.layernorm", layernorm(w.X, ln2w, ln2b, w.XN, (int)g.M, D, 1e-6f, 0, 0, 0, st));
     { GemmParams p = base_params(g.M, 4 * D, D); p.bias = bfc1; p.act = ACT_GELU; p.out_h = w.H1; p.out_h_ld = 4 * D;
       MK_TRY(gemm(h, "vit.fc1", EPI_STORE_H, w.XN, g.M, D, wfc1, 4 * D, D, p, st)); }
     { GemmParams p = base_params(g.M, D, 4 * D); p.bias = bfc2; p.gamma = ls2; p.out_f = w.X; p.out_f_ld = D;
-      const bool fuse_next = fuse_ln && i + 1 < c.depth;
-      if (fuse_next) {
-        const std::string nb = "blk" + std::to_string(i + 1) + ".";
-        p.aux = L.f(nb + "ln1.w", D); p.beta = L.f(nb + "ln1.b", D); p.out_h = w.XN; p.out_h_ld = D; p.eps = 1e-6f;
-        if (!L.ok) return MK_ERR_MISSING_TENSOR;
-      }
-      MK_TRY(gemm(h, "vit.fc2", fuse_next ? EPI_RESID_LN : EPI_RESID_F, w.H1, g.M, 4 * D, wfc2, D, 4 * D, p, st)); }
+      MK_TRY(gemm(h, "vit.fc2", EPI_RESID_F, w.H1, g.M, 4 * D, wfc2, D, 4 * D, p, st)); }
   }
   return MK_OK;
 }

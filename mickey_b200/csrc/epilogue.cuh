@@ -181,113 +181,12 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, int g, int m
 // k ^ h with h = 2 (r % 4) + ((r ^ r / 4 ^ k / 8) & 1) < 8, a permutation of the row's chunks that keeps 16-byte
 // accesses whole.  Every access pattern of the block is free of bank conflicts: the park's float2 stores (rows r..r+3,
 // chunks 2m, 2m + 1 per half-warp), acc_chunk's float4 reads (one chunk of rows 0..7 per quarter-warp), epilogue_rows'
-// float4 reads (chunks 0, 2, .., 14 of one row, or 0, 2, 4, 6 of rows 2t, 2t + 1) and the float2 rows of EPI_RESID_LN.
+// float4 reads (chunks 0, 2, .., 14 of one row, or 0, 2, 4, 6 of rows 2t, 2t + 1).
 // A row stride of W + 4 left the park's stores 2-way conflicted while the tensor cores wait for it.
 template <int W> __device__ __forceinline__ int acc_idx(int r, int c) {
   const int k = c >> 2;
   const int h = 2 * (r & 3) + ((r ^ (r >> 2) ^ (k >> 3)) & 1);
   return r * W + ((k ^ h) << 2) + (c & 3);
-}
-
-template <int CPL> struct VecF;
-template <> struct VecF<1> { using T = float; };
-template <> struct VecF<2> { using T = float2; };
-
-template <int CPL> __device__ __forceinline__ void ld_f(const float* p, float (&v)[CPL]) {
-  if constexpr (CPL == 2) { const float2 t = *reinterpret_cast<const float2*>(p); v[0] = t.x; v[1] = t.y; } else { v[0] = *p; }
-}
-template <int CPL> __device__ __forceinline__ void ldg_f(const float* p, float (&v)[CPL]) {
-  if constexpr (CPL == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); v[0] = t.x; v[1] = t.y; } else { v[0] = __ldg(p); }
-}
-template <int CPL> __device__ __forceinline__ void st_f(float* p, const float (&v)[CPL]) {
-  if constexpr (CPL == 2) { *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]); } else { *p = v[0]; }
-}
-template <int CPL> __device__ __forceinline__ void st_h(__half* p, const float (&v)[CPL]) {
-  if constexpr (CPL == 2) { *reinterpret_cast<__half2*>(p) = __floats2half2_rn(v[0], v[1]); } else { *p = __float2half_rn(v[0]); }
-}
-template <int CPL> __device__ __forceinline__ void ld_h(const __half* p, float (&v)[CPL]) {
-  if constexpr (CPL == 2) { const float2 t = __half22float2(*reinterpret_cast<const __half2*>(p)); v[0] = t.x; v[1] = t.y; }
-  else { v[0] = __half2float(*p); }
-}
-
-// ---- fused residual + LayerNorm epilogue (EPI_RESID_LN) -------------------------------------------------
-// A warp owns 32 rows x 64 columns of the tile (lane = column pair).  Row statistics are needed per ROW, the
-// layout is per COLUMN: every lane first accumulates its own partial of all 32 rows, then a recursive-halving
-// exchange (31 shuffles instead of 32 x 5) leaves the total of row r in lane r.  The order of the additions is fixed.
-__device__ __forceinline__ float warp_rowsum32(float (&part)[32], int lane) {
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) {
-    const bool upper = (lane & o) != 0;
-#pragma unroll
-    for (int i = 0; i < o; ++i) {
-      const float send = upper ? part[i] : part[i + o];
-      const float keep = upper ? part[i + o] : part[i];
-      part[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-    }
-  }
-  return part[0];
-}
-
-// pass 1: x = out_f + gamma * (acc + bias) -> out_f (fp32, in place) and back into the staging block; returns the
-// sum of row (lane) over the warp's 64 columns.  Rows at or beyond p.M contribute zeros and are not stored.
-__device__ __forceinline__ float resid_ln_pass1(const GemmParams& p, int row0, int lane, int col_base, float* stage) {
-  constexpr int RB = 8;
-  const int col = col_base + lane * 2;
-  const float2 bias = __ldg(reinterpret_cast<const float2*>(p.bias + col)), gam = __ldg(reinterpret_cast<const float2*>(p.gamma + col));
-  const int rows = min(32, p.M - row0);
-  float part[32];
-#pragma unroll
-  for (int r0 = 0; r0 < 32; r0 += RB) {
-    float2 v[RB], x[RB];
-#pragma unroll
-    for (int i = 0; i < RB; ++i) {
-      const int r = r0 + i;
-      v[i] = *reinterpret_cast<const float2*>(stage + acc_idx<64>(r, lane * 2));
-      x[i] = make_float2(0.f, 0.f);
-      if (r < rows) x[i] = *reinterpret_cast<const float2*>(p.out_f + (size_t)(row0 + r) * p.out_f_ld + col);
-    }
-#pragma unroll
-    for (int i = 0; i < RB; ++i) {
-      const int r = r0 + i;
-      float2 y = make_float2(0.f, 0.f);
-      if (r < rows) {
-        y.x = fmaf(gam.x, v[i].x + bias.x, x[i].x); y.y = fmaf(gam.y, v[i].y + bias.y, x[i].y);
-        *reinterpret_cast<float2*>(p.out_f + (size_t)(row0 + r) * p.out_f_ld + col) = y;
-      }
-      *reinterpret_cast<float2*>(stage + acc_idx<64>(r, lane * 2)) = y;
-      part[r] = y.x + y.y;
-    }
-  }
-  return warp_rowsum32(part, lane);
-}
-
-// pass 2: sum over the warp's 64 columns of (x - mean_row)^2; mean_l holds the mean of row (lane)
-__device__ __forceinline__ float resid_ln_pass2(int lane, const float* stage, float mean_l) {
-  float part[32];
-#pragma unroll
-  for (int r = 0; r < 32; ++r) {
-    const float2 x = *reinterpret_cast<const float2*>(stage + acc_idx<64>(r, lane * 2));
-    const float mean = __shfl_sync(0xffffffffu, mean_l, r);
-    const float d0 = x.x - mean, d1 = x.y - mean;
-    part[r] = d0 * d0 + d1 * d1;
-  }
-  return warp_rowsum32(part, lane);
-}
-
-// pass 3: out_h = (x - mean) * rstd * ln_w + ln_b   (ln_w = p.aux, ln_b = p.beta)
-__device__ __forceinline__ void resid_ln_pass3(const GemmParams& p, int row0, int lane, int col_base, const float* stage,
-                                               float mean_l, float rstd_l) {
-  const int col = col_base + lane * 2;
-  const float2 w = __ldg(reinterpret_cast<const float2*>(p.aux + col)), b = __ldg(reinterpret_cast<const float2*>(p.beta + col));
-  const int rows = min(32, p.M - row0);
-#pragma unroll 8
-  for (int r = 0; r < 32; ++r) {
-    const float2 x = *reinterpret_cast<const float2*>(stage + acc_idx<64>(r, lane * 2));
-    const float mean = __shfl_sync(0xffffffffu, mean_l, r), rstd = __shfl_sync(0xffffffffu, rstd_l, r);
-    if (r < rows)
-      *reinterpret_cast<__half2*>(p.out_h + (size_t)(row0 + r) * p.out_h_ld + col) =
-          __floats2half2_rn((x.x - mean) * rstd * w.x + b.x, (x.y - mean) * rstd * w.y + b.y);
-  }
 }
 
 // Lane layout of the staged epilogue: a lane owns EIGHT consecutive columns (one 16-byte fp16 store, two 16-byte fp32
@@ -483,6 +382,20 @@ __device__ __forceinline__ float warp_colmax32(float (&part)[32], int lane) {
       const float send = upper ? part[i] : part[i + o];
       const float keep = upper ? part[i + o] : part[i];
       part[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, o));
+    }
+  }
+  return part[0];
+}
+
+__device__ __forceinline__ float warp_rowsum32(float (&part)[32], int lane) {
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) {
+    const bool upper = (lane & o) != 0;
+#pragma unroll
+    for (int i = 0; i < o; ++i) {
+      const float send = upper ? part[i] : part[i + o];
+      const float keep = upper ? part[i + o] : part[i];
+      part[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
     }
   }
   return part[0];

@@ -142,7 +142,7 @@ static const OutMaps& no_out_maps() { static OutMaps z = {}; return z; }
 // ---- SIMT debug kernel --------------------------------------------------------------------------------
 // Same operand addressing and the same epilogues as the wgmma kernel, computed with plain FFMA.  It is
 // NOT a product path: it exists so that a GPU test can tell a wgmma/TMA descriptor bug from an epilogue
-// bug (tests/test_gpu_ops.py runs both and compares), selectable with MICKEY_GEMM_IMPL=simt.
+// bug (tests/test_gpu_ops.py runs both and compares); tests reach it through impl = 2 (GEMM_IMPL_SIMT).
 template <int BN, int EPI>
 __global__ void __launch_bounds__(128)
 gemm_simt_kernel(const __half* __restrict__ A, long long a_rows, long long lda, const __half* __restrict__ B,
@@ -214,15 +214,6 @@ bool pdl_enabled() {
 }
 
 // ---- dispatch -----------------------------------------------------------------------------------------
-static bool use_simt() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MICKEY_GEMM_IMPL");
-    v = (e && strcmp(e, "simt") == 0) ? 1 : 0;
-  }
-  return v == 1;
-}
-
 int sm_count() {
   static int n[64] = {0};
   int dev = 0;
@@ -233,10 +224,9 @@ int sm_count() {
 }
 
 // Persistent instantiations get one CTA per SM (fewer if there are fewer tiles); the one-tile-per-CTA ones one CTA per
-// tile.  EPI_RESID_LN: each row of tiles (gemm_tile keeps it consecutive) forms one thread-block cluster, which
-// exchanges row statistics through DSMEM.  PAIR: two-CTA clusters, as many as can be resident at once (fewer if there
-// are fewer tile pairs).  That count comes from the occupancy API, not from SMs / 2: a cluster's CTAs share a GPC, and
-// a GPC with an odd number of free SMs leaves one idle; a grid beyond the resident clusters would run a second wave.
+// tile.  PAIR: two-CTA clusters, as many as can be resident at once (fewer if there are fewer tile pairs).  That count
+// comes from the occupancy API, not from SMs / 2: a cluster's CTAs share a GPC, and a GPC with an odd number of free
+// SMs leaves one idle; a grid beyond the resident clusters would run a second wave.
 template <int BN, int EPI, int STAGES, bool PERSISTENT, bool PAIR = false>
 static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream,
                      const OutMaps& om = no_out_maps()) {
@@ -248,9 +238,9 @@ static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmP
   cfg.blockDim = dim3(gemm_threads<PERSISTENT>()); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   int n_attr = 0;
-  if constexpr (EPI == EPI_RESID_LN || PAIR) {
+  if constexpr (PAIR) {
     attr[n_attr].id = cudaLaunchAttributeClusterDimension;
-    attr[n_attr].val.clusterDim.x = PAIR ? 2 : p.N / BN; attr[n_attr].val.clusterDim.y = 1; attr[n_attr++].val.clusterDim.z = 1;
+    attr[n_attr].val.clusterDim.x = 2; attr[n_attr].val.clusterDim.y = 1; attr[n_attr++].val.clusterDim.z = 1;
   }
   cfg.attrs = attr;
   cfg.numAttrs = n_attr;
@@ -293,11 +283,7 @@ static bool persistent_grid(int tiles) { return tiles > 8 * sm_count(); }
 template <int BN, int EPI>
 static int launch_one(const GemmOperand& A, const GemmOperand& B, const GemmParams& p, cudaStream_t stream, int impl) {
   const int tiles = gemm_tile_count<BN>(p);
-  if constexpr (EPI == EPI_RESID_LN) {
-    if (impl == GEMM_IMPL_SIMT || BN != 128 || p.N / BN > 8 || p.groups != 1) { set_last_error("EPI_RESID_LN: wgmma path, N <= 1024, one group"); return MK_ERR_UNSUPPORTED; }
-  }
   if (impl == GEMM_IMPL_SIMT) {
-    if constexpr (EPI != EPI_RESID_LN)
     MK_CUDA_CHECK(launch_k(gemm_simt_kernel<BN, EPI>, dim3(tiles), dim3(128), 0, stream, reinterpret_cast<const __half*>(A.ptr),
                            (long long)A.rows, (long long)A.ld, reinterpret_cast<const __half*>(B.ptr), (long long)B.rows,
                            (long long)B.ld, p));
@@ -344,18 +330,7 @@ static int launch_bn(int bn, const GemmOperand& A, const GemmOperand& B, const G
   return MK_ERR_INVALID;
 }
 
-// Would launch_gemm run a [M, N] x K RESID_F GEMM on a one-tile kernel (so that LayerNorm can be fused into it)?
-bool gemm_resid_ln_supported(int M, int N, int k_chunks) {
-  // opt-in (MICKEY_FUSE_LN=1): the fused epilogue removes a LayerNorm launch per block but adds three cluster barriers
-  // and two extra passes over the staged tile.
-  (void)M; (void)k_chunks;
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("MICKEY_FUSE_LN"); on = (e && e[0] == '1') ? 1 : 0; }
-  return on && !use_simt() && N % 128 == 0 && N <= 1024;
-}
-
 int launch_gemm(int epi, const GemmOperand& A, const GemmOperand& B, const GemmParams& p, cudaStream_t stream, int impl) {
-  if (impl == GEMM_IMPL_DEFAULT) impl = use_simt() ? GEMM_IMPL_SIMT : GEMM_IMPL_TC;
   if (p.k_chunks <= 0 || p.M <= 0 || p.N <= 0 || p.groups <= 0) { set_last_error("bad GEMM shape"); return MK_ERR_INVALID; }
   const bool matcher = (epi == EPI_LSE || epi == EPI_DUAL);
   if (matcher && impl == GEMM_IMPL_SIMT) { set_last_error("the matcher epilogues run on the wgmma kernel only"); return MK_ERR_UNSUPPORTED; }
@@ -365,14 +340,9 @@ int launch_gemm(int epi, const GemmOperand& A, const GemmOperand& B, const GemmP
   int bn = (matcher || p.N % 128 == 0) ? 128 : 64;
   if (!matcher && p.N % bn) { set_last_error("GEMM N=%d not tileable", p.N); return MK_ERR_INVALID; }
   if (epi == EPI_LN && p.N != 128) { set_last_error("EPI_LN needs N == 128"); return MK_ERR_INVALID; }
-  if (epi == EPI_RESID_LN && (p.N % 128 || p.N > 1024 || p.groups != 1 || !p.aux || !p.beta || !p.out_h || !p.out_f)) {
-    set_last_error("EPI_RESID_LN needs N % 128 == 0, N <= 1024, one group, LN weight (aux), LN bias (beta), out_f and out_h");
-    return MK_ERR_INVALID;
-  }
   switch (epi) {
     case EPI_STORE_H: return launch_bn<EPI_STORE_H>(bn, A, B, p, stream, impl);
     case EPI_RESID_F: return launch_bn<EPI_RESID_F>(bn, A, B, p, stream, impl);
-    case EPI_RESID_LN: return launch_one<128, EPI_RESID_LN>(A, B, p, stream, impl);
     case EPI_PATCH:   return launch_bn<EPI_PATCH>(bn, A, B, p, stream, impl);
     case EPI_CONV:    return launch_bn<EPI_CONV>(bn, A, B, p, stream, impl);
     case EPI_STORE_F: return launch_bn<EPI_STORE_F>(bn, A, B, p, stream, impl);

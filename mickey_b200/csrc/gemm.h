@@ -9,6 +9,7 @@ struct GemmOperand {       // a row-major fp16 matrix [rows, cols] with leading 
   long long rows, cols, ld;
 };
 
+// GEMM_IMPL_DEFAULT and GEMM_IMPL_TC run the wgmma kernel; GEMM_IMPL_SIMT runs the SIMT debug kernel.
 // GEMM_IMPL_TC_PAIRED / _UNPAIRED run the persistent kernel with or without two-CTA pairs on every grid whose epilogue
 // it serves (other epilogues run as GEMM_IMPL_TC), whatever the grid size: a test or a benchmark can set the two side
 // by side.  The default picks the paired kernel for grids of more than 8 tiles per SM.
@@ -24,8 +25,6 @@ int make_tensor_map_out_f16(CUtensorMap* map, void* ptr, long long groups, long 
 int sm_count();            // SMs of the current device
 int launch_gemm(int epi, const GemmOperand& A, const GemmOperand& B, const GemmParams& p, cudaStream_t stream,
                 int impl = GEMM_IMPL_DEFAULT);
-// true when launch_gemm would put a [M, N] x (64 k_chunks) residual GEMM on a one-tile kernel, i.e. EPI_RESID_LN may be used
-bool gemm_resid_ln_supported(int M, int N, int k_chunks);
 const char* last_error();
 
 }  // namespace mk

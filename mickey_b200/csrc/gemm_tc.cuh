@@ -17,10 +17,10 @@
 //
 // The other instantiations (!PERSISTENT) run one tile per CTA (grid = tiles, the same loop runs once) with 288 threads:
 // the MMA warps park the accumulators in the idle ring and run the epilogue themselves, warp 8 is the producer.  They
-// serve EPI_DUAL (its TMA-store staging takes the room of a second buffer), EPI_RESID_LN (a thread-block cluster is one
-// row of tiles), EPI_LN (its epilogue needs more registers than the persistent epilogue warps have) and grids too small
-// to keep a persistent CTA per SM busy: a 3-stage ring (two CTAs per SM, one CTA's epilogue under the other's main loop,
-// except for the LayerNorm epilogues) or, for at most ~1.25 tiles per SM, a deep ring.
+// serve EPI_DUAL (its TMA-store staging takes the room of a second buffer), EPI_LN (its epilogue needs more registers
+// than the persistent epilogue warps have) and grids too small to keep a persistent CTA per SM busy: a 3-stage ring (two
+// CTAs per SM, one CTA's epilogue under the other's main loop, except for EPI_LN) or, for at most ~1.25 tiles per SM, a
+// deep ring.
 //
 // The K loop walks `k_chunks` 64-element chunks.  For convolutions a chunk also selects a filter tap:
 // the A tile of tap t is the same 2-D tensor read at row offset tap_shift[t] (negative / overflowing
@@ -42,7 +42,7 @@ constexpr int GEMM_WARP_EPI = 8;
 template <int BN> constexpr int ring_stages() { return BN == 128 ? 4 : 6; }
 template <int BN> constexpr int shallow_stages() { return BN == 128 ? 3 : 4; }
 template <int BN> constexpr int deep_stages() { return BN == 128 ? 6 : 8; }
-template <int EPI> constexpr bool persistent_epilogue() { return EPI != EPI_DUAL && EPI != EPI_RESID_LN && EPI != EPI_LN; }
+template <int EPI> constexpr bool persistent_epilogue() { return EPI != EPI_DUAL && EPI != EPI_LN; }
 template <bool PERSISTENT> constexpr int gemm_threads() { return PERSISTENT ? 640 : 288; }
 template <bool PERSISTENT> constexpr int gemm_warp_tma() { return PERSISTENT ? 16 : 8; }
 
@@ -65,14 +65,14 @@ constexpr int region_bytes() {
   return ring_bytes<BN, STAGES>() > acc_tile_offset<BN, EPI, STAGES, PERSISTENT>() + acc_tile_bytes<BN>()
              ? ring_bytes<BN, STAGES>() : acc_tile_offset<BN, EPI, STAGES, PERSISTENT>() + acc_tile_bytes<BN>();
 }
-// + 1024 alignment slack + 256 barriers + 2 KB row statistics (EPI_RESID_LN)
+// + 1024 alignment slack + 256 barriers
 template <int BN, int EPI, int STAGES, bool PERSISTENT> constexpr int gemm_smem_bytes() {
-  return region_bytes<BN, EPI, STAGES, PERSISTENT>() + 1024 + 256 + 2048;
+  return region_bytes<BN, EPI, STAGES, PERSISTENT>() + 1024 + 256;
 }
-// Two one-tile CTAs per SM when their shared memory allows it, except for the LayerNorm epilogues: at two CTAs per SM
-// a thread has 96 registers, and they spill below about 140.
+// Two one-tile CTAs per SM when their shared memory allows it, except for EPI_LN: at two CTAs per SM a thread has 96
+// registers, and its epilogue spills below about 140.
 template <int BN, int EPI, int STAGES, bool PERSISTENT> constexpr int gemm_ctas_per_sm() {
-  return !PERSISTENT && EPI != EPI_LN && EPI != EPI_RESID_LN && gemm_smem_bytes<BN, EPI, STAGES, PERSISTENT>() <= 113 * 1024 ? 2 : 1;
+  return !PERSISTENT && EPI != EPI_LN && gemm_smem_bytes<BN, EPI, STAGES, PERSISTENT>() <= 113 * 1024 ? 2 : 1;
 }
 
 // ---- tile order ----------------------------------------------------------------------------------------
@@ -81,7 +81,7 @@ template <int BN, int EPI, int STAGES, bool PERSISTENT> constexpr int gemm_ctas_
 // outermost, so a group's tiles stay together.  The ViT GEMMs have M in the ~1000 tiles and A far larger than the
 // 50 MB L2 while all of B is a few MB: the ~132 tiles in flight at once then cover a few complete rows of tiles, every
 // A row-panel is read from HBM about once and B stays resident in L2.  An M-fastest order would instead stream A once
-// per column of N-tiles.  EPI_RESID_LN relies on a row of tiles being consecutive: its clusters are those rows.
+// per column of N-tiles.
 // MT = 2 (the paired persistent kernel) walks the same order over pairs of M-tiles 2 mp, 2 mp + 1: the CTA of cluster
 // rank r takes M-tile 2 mp + r.  With an odd M-tile count the last pair's rank-1 tile starts at or beyond M.
 struct GemmTile { int g, m0, n0, n_tile; };
@@ -209,21 +209,9 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t desc_a, 
   else wgmma_m64n64k16(d, desc_a, desc_b, scale_d);
 }
 
-// ---- thread-block cluster helpers (EPI_RESID_LN) -------------------------------------------------------
+// ---- thread-block cluster barrier (PAIR) ---------------------------------------------------------------
 __device__ __forceinline__ void cluster_sync_all() {     // every thread of every CTA of the cluster
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_size() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ float ld_dsmem_f32(uint32_t local_smem_addr, uint32_t cta_rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local_smem_addr), "r"(cta_rank));
-  float v;
-  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
-  return v;
 }
 
 // ---- tile epilogue -----------------------------------------------------------------------------------
@@ -243,7 +231,7 @@ __device__ __forceinline__ void acc_chunk(const float* acc, int q, int lane, int
 
 template <int BN, int EPI>
 __device__ __forceinline__ void tile_epilogue(const GemmParams& p, const OutMaps& om, int g, int m0, int n0, int n_tile, int q, int half,
-                                              int lane, float* acc, float* red, uint32_t red_saddr, float* dual_stage, float* dual_aux) {
+                                              int lane, float* acc, float* dual_stage, float* dual_aux) {
   constexpr int CHUNKS = BN / 32;
   constexpr int W = BN / 2;                             // columns owned by this warp
   constexpr int CPH = CHUNKS / 2;                       // chunks per half
@@ -269,27 +257,6 @@ __device__ __forceinline__ void tile_epilogue(const GemmParams& p, const OutMaps
     }
     const float rstd = rsqrtf(sq * (1.0f / BN) + p.eps);
     epilogue_rows<EPI_LN, W>(p, g, m0 + q * 32, lane, n0 + half * W, stage, mean, rstd);
-  } else if constexpr (EPI == EPI_RESID_LN) {
-    // `red` = this CTA's float[2 statistics][2 column halves][128 rows]; the CTAs of the cluster hold the other
-    // 128-column tiles of the same rows
-    static_assert(BN == 128, "EPI_RESID_LN: 128-wide tiles");
-    const int row0 = m0 + q * 32, col_base = n0 + half * 64, slot = half * 128 + q * 32 + lane;
-    const uint32_t n_cta = cluster_size();
-    const float inv_n = 1.0f / (float)p.N;
-    red[slot] = resid_ln_pass1(p, row0, lane, col_base, stage);
-    cluster_sync_all();
-    float tot = 0.f;
-    for (uint32_t c = 0; c < n_cta; ++c)
-      tot += ld_dsmem_f32(red_saddr + (q * 32 + lane) * 4, c) + ld_dsmem_f32(red_saddr + (128 + q * 32 + lane) * 4, c);
-    const float mean = tot * inv_n;
-    red[256 + slot] = resid_ln_pass2(lane, stage, mean);
-    cluster_sync_all();
-    float tot2 = 0.f;
-    for (uint32_t c = 0; c < n_cta; ++c)
-      tot2 += ld_dsmem_f32(red_saddr + (256 + q * 32 + lane) * 4, c) + ld_dsmem_f32(red_saddr + (384 + q * 32 + lane) * 4, c);
-    const float rstd = rsqrtf(tot2 * inv_n + p.eps);
-    resid_ln_pass3(p, row0, lane, col_base, stage, mean, rstd);
-    cluster_sync_all();                  // no CTA may exit while a peer can still read its statistics
   } else if constexpr (EPI == EPI_LSE) {
     static_assert(BN == 128, "matcher epilogues: 128-wide tiles");
     const bool row_ok = m < p.n_valid;
@@ -377,13 +344,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // swizzle-128B tiles need 1024-byte alignment
-  // full[S], empty[S], acc_full, acc_empty; then 2 KB of row statistics
+  // full[S], empty[S], acc_full, acc_empty
   const uint32_t bar_base = base + region_bytes<BN, EPI, STAGES, PERSISTENT>();
   const uint32_t full_bar0 = bar_base;
   const uint32_t empty_bar0 = bar_base + 8 * STAGES;
   const uint32_t acc_full_bar = bar_base + 16 * STAGES;         // staging buffer holds a tile (256 MMA threads arrive)
   const uint32_t acc_empty_bar = acc_full_bar + 8;              // the epilogue is done with it (256 epilogue threads)
-  const uint32_t red_saddr = bar_base + 256;
   uint8_t* const gbase = smem_raw + (base - raw);
   float* const acc = reinterpret_cast<float*>(gbase + acc_tile_offset<BN, EPI, STAGES, PERSISTENT>());
 
@@ -435,8 +401,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     __syncwarp();
     pdl_trigger();
-    // EPI_RESID_LN: every thread of every CTA of the cluster takes part in the three cluster barriers
-    if constexpr (EPI == EPI_RESID_LN) { cluster_sync_all(); cluster_sync_all(); cluster_sync_all(); }
     // a pair: no CTA may exit while its peer can still multicast into its ring or arrive on its barriers
     if constexpr (PAIR) cluster_sync_all();
     return;
@@ -495,7 +459,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         consumer_sync();
         const GemmTile tile = gemm_tile<BN>(p, t);
         tile_epilogue<BN, EPI>(p, om, tile.g, tile.m0, tile.n0, tile.n_tile, warp & 3, warp >> 2, lane, acc,
-                               reinterpret_cast<float*>(smem_raw + (red_saddr - raw)), red_saddr,
                                reinterpret_cast<float*>(gbase + warp * DUAL_STAGE_BYTES),
                                reinterpret_cast<float*>(gbase + 8 * DUAL_STAGE_BYTES) + warp * 64);
       } else {
@@ -520,7 +483,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // the rank-1 tile of the last pair of an odd M-tile count lies wholly beyond M: it stores nothing
     if (tile.m0 < p.M)
       tile_epilogue<BN, EPI>(p, om, tile.g, tile.m0, tile.n0, tile.n_tile, ew & 3, ew >> 2, lane, acc,
-                             reinterpret_cast<float*>(smem_raw + (red_saddr - raw)), red_saddr,
                              reinterpret_cast<float*>(gbase + ew * DUAL_STAGE_BYTES),
                              reinterpret_cast<float*>(gbase + 8 * DUAL_STAGE_BYTES) + ew * 64);
     mbar_arrive(acc_empty_bar);

@@ -28,10 +28,7 @@ PATCH = 14
 def nn_pitch(N: int) -> int:
     """Row pitch (floats) of the N x N outputs the engine allocates: N rounded up to 32, so that every row starts on a
     128-byte line and the matcher's outputs can leave through TMA tensor stores (N = 1938 rows are only 8-byte aligned).
-    The tensors handed out are the [.., :N] views; MICKEY_NN_CONTIGUOUS=1 keeps the reference's contiguous layout."""
-    import os
-    if os.environ.get("MICKEY_NN_CONTIGUOUS") == "1":
-        return N
+    The tensors handed out are the [.., :N] views."""
     return (N + 31) // 32 * 32
 
 

@@ -5,7 +5,7 @@ import torch
 
 from mickey_b200 import _lib
 
-EPI = dict(STORE_H=0, RESID_F=1, PATCH=2, CONV=3, STORE_F=4, LN=5, LSE=6, DUAL=7, RESID_LN=8)
+EPI = dict(STORE_H=0, RESID_F=1, PATCH=2, CONV=3, STORE_F=4, LN=5, LSE=6, DUAL=7)
 IMPL = dict(default=0, tc=1, simt=2)
 
 

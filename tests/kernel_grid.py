@@ -15,7 +15,7 @@ from dataclasses import dataclass, field
 from typing import Optional
 
 MATCHER = ("LSE", "DUAL")
-ONE_TILE_ONLY = ("DUAL", "LN", "RESID_LN")             # gemm_tc.cuh persistent_epilogue() is false for these
+ONE_TILE_ONLY = ("DUAL", "LN")                         # gemm_tc.cuh persistent_epilogue() is false for these
 REGIMES = ("persistent", "deep", "shallow")
 # ring depths (gemm_tc.cuh ring_stages / deep_stages / shallow_stages), by BN
 STAGES = {"persistent": {128: 4, 64: 6}, "deep": {128: 6, 64: 8}, "shallow": {128: 3, 64: 4}}
@@ -40,7 +40,7 @@ class GemmLaunch:
 
     @property
     def bn(self) -> int:
-        return 128 if (self.epi in MATCHER or self.epi in ("LN", "RESID_LN") or self.N % 128 == 0) else 64
+        return 128 if (self.epi in MATCHER or self.epi == "LN" or self.N % 128 == 0) else 64
 
     @property
     def m_tiles(self) -> int:
@@ -220,10 +220,6 @@ def gemm_cases(sms: int) -> list:
     add("ln_shared_a_shallow", "LN", 3 * 30 * 31, 128, 3, "shallow", groups=2, group_fast=True, a_col_base=64,
         b_row_group_off=128, extra=dict(n_img=3, h2=30, w2=31))
 
-    # ---- EPI_RESID_LN: clusters of 1..8 CTAs (one row of tiles), ragged last row of tiles ----
-    for c, (M, k) in enumerate(((130, 2), (700, 6), (1000, 4), (515, 3), (3000, 8), (777, 5), (2000, 2), (333, 12)), 1):
-        L = GemmLaunch("RESID_LN", M, 128 * c, k, sms=s)
-        add(f"resid_ln_cluster{c}", "RESID_LN", M, 128 * c, k, L.regime, bias=True)
     # ---- the matcher: EPI_LSE -> mk_op_matcher_reduce -> EPI_DUAL ----
     for n, B, confs in ((2, 3, ((0.0, False, False), (1.001, True, True))),
                         (127, 2, ((1.001, False, False), (0.0, True, True))),
@@ -239,12 +235,6 @@ def gemm_cases(sms: int) -> list:
             dual = GemmLaunch("DUAL", n, n, 6, B, out_tma=tma, sms=s)
             add(f"dual_{tag}", "DUAL", n, n, 6, dual.regime, groups=B, a_row_group_off=n, b_row_group_off=n, extra=ex)
     return cases
-
-
-# EPI_RESID_LN at the shapes of attn.proj and mlp.fc2: (name, M, N, K)
-RESID_LN_PRODUCTION = (("C2_vits_proj", 3878, 384, 384), ("C2_vits_fc2", 3878, 384, 1536),
-                       ("C3_vitb_proj", 64 * 1939, 768, 768), ("C3_vitb_fc2", 64 * 1939, 768, 3072),
-                       ("L_vitl_proj", 2 * 1939, 1024, 1024), ("L_vitl_fc2", 2 * 1939, 1024, 4096))
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -297,9 +287,6 @@ def requirements(sms: int) -> dict:
     for mask in (0x0, 0x7, 0x8, 0xF):
         req[f"CONV pad ring, shortcut, aux_group_mask {mask:#x}"] = (
             lambda c, m=mask: c.epi == "CONV" and c.extra["pad"] and c.extra.get("mask") == m)
-    for cl in range(1, 9):
-        req[f"RESID_LN cluster of {cl}, ragged last row of tiles"] = (
-            lambda c, n=cl: c.epi == "RESID_LN" and c.N == 128 * n and c.M % 128 != 0)
     for n in (2, 127, 128, 129, 1938):
         req[f"matcher n_valid {n}"] = lambda c, n=n: c.epi == "DUAL" and c.M == n
     for bound in (False, True):

@@ -55,3 +55,13 @@ def test_every_ctypes_struct_matches_the_library(name, struct):
 
 def test_sizeof_an_unknown_struct_is_minus_one():
     assert _lib.load().mk_sizeof(b"nope") == -1
+
+
+@pytest.mark.parametrize("epi", [8, 9])
+def test_gemm_rejects_an_unknown_epilogue_before_any_launch(epi):
+    """The epilogue list ends at 7 (DUAL): a well-formed GEMM with any other epi is refused on the host."""
+    lib = _lib.load()
+    g = _lib.MkGemmArgs()
+    g.epi, g.M, g.N, g.k_chunks, g.chunks_per_tap, g.num_taps, g.groups = epi, 128, 128, 1, 1, 1, 1
+    assert lib.mk_op_gemm(ctypes.byref(g), None) == -1
+    assert lib.mk_last_error().decode() == f"unknown epilogue {epi}"

@@ -42,13 +42,13 @@ def test_sine_table_padded_is_the_oracle(name):
 
 @pytest.mark.parametrize("name", sorted(st.GEOMETRIES))
 def test_pitch_and_sampler_mode(name, monkeypatch):
-    monkeypatch.delenv("MICKEY_NN_CONTIGUOUS", raising=False)
+    monkeypatch.setenv("MICKEY_NN_CONTIGUOUS", "1")           # has no effect: the engine's N x N pitch is always padded
     _, _, H, W, _, _, _ = st.GEOMETRIES[name]
     (gh, gw), N, pitch, mode = st.GEOMETRY_PATHS[name]
     assert (H // 14, W // 14) == (gh, gw) and gh * gw == N
     assert nn_pitch(N) == pitch
     assert st.sampler_mode(N, pitch) == mode
-    assert st.sampler_mode(N, N) == ("FLAT_VEC" if N * N % 4 == 0 else "SCALAR")       # MICKEY_NN_CONTIGUOUS=1
+    assert st.sampler_mode(N, N) == ("FLAT_VEC" if N * N % 4 == 0 else "SCALAR")       # caller tensors at pitch N
     assert st.sampler_mode(N, pitch, aligned=False) == "SCALAR"
 
 

@@ -427,78 +427,6 @@ def test_gemm_layernorm_epilogue():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# RESID_LN: the cluster-fused residual + LayerNorm
-# ---------------------------------------------------------------------------------------------------------------
-def _resid_ln(name, M, N, K, sms, family):
-    L = kg.GemmLaunch("RESID_LN", M, N, K // 64, sms=sms)
-    seed = _seed(name)
-    A = _randn((M, K), seed)
-    B = _randn((N, K), seed + 1, 1 / math.sqrt(K))
-    bias = _randn((N,), seed + 2, 0.1, torch.float32)
-    gamma = _randn((N,), seed + 3, 0.5, torch.float32)
-    x0 = _randn((M, N), seed + 4, 1.0, torch.float32)
-    ln_w = _randn((N,), seed + 5, 1.0, torch.float32)
-    ln_b = _randn((N,), seed + 6, 0.3, torch.float32)
-    rows = L.m_tiles * 128 + 8
-    of = torch.full((rows, N + 32), SENT, device=DEV)
-    of[:M, :N] = x0
-    oh = torch.full((rows, N + 32), SENT, dtype=torch.float16, device=DEV)
-    gemm("RESID_LN", A, B, M, N, K, bias=bias, gamma=gamma, out_f=of, out_f_ld=N + 32, aux=ln_w, beta=ln_b, out_h=oh,
-         out_h_ld=N + 32, eps=1e-6)
-    torch.cuda.synchronize()
-    written = torch.zeros(rows, N + 32, dtype=torch.bool, device=DEV)
-    written[:M, :N] = True
-    _assert_sentinels("fp32 residual", of, written)
-    _assert_sentinels("fp16 LayerNorm", oh, written)
-    a, w = A.double(), B.double()
-    pre = a @ w.t()
-    acc = ew.gemm_acc_bound(K, a.abs() @ w.abs().t())
-    del a
-    b, gm, x0d = bias.double(), gamma.double(), x0.double()
-    x_ref = x0d + gm * (pre + b)
-    e_x = gm.abs() * (acc + ew.epilogue_terms(pre, b)) + ew.epilogue_terms(x_ref, x0d) + ew.out_rounding(x_ref, False)
-    del acc
-
-    def post(p, rs, cs):
-        return x0d[rs, cs] + gm[cs] * (p + b[cs])
-
-    def drop(g, rs, cs):
-        return A[rs, K - 64:].double() @ B[cs, K - 64:].double().t()
-
-    xm = _tile_mutations(L, 0, [pre], post, drop, x_ref)
-    where = ew.Where(lambda idx: (int(idx[0]), 0, int(idx[1])), ew.Rows(), L)
-    r1 = ew.check(f"{name} fp32 residual", of[:M, :N], x_ref, e_x.clamp_min(1e-30), where, xm)
-    lw, lb = ln_w.double(), ln_b.double()
-    y, yb = ew.ln_bound(x_ref, e_x, lw, lb, 1e-6)
-    ym = []
-    for mu in xm:                           # the same bugs seen through the row statistics
-        rs, cs = mu.idx
-        xr = x_ref[rs].clone()
-        xr[:, cs] = mu.values
-        ym.append(ew.Mutation(mu.label, (rs, slice(None)), ew.ln_bound(xr, 0.0, lw, lb, 1e-6)[0]))
-    r2 = ew.check(f"{name} fp16 LayerNorm", oh[:M, :N], y, (yb + ew.out_rounding(y, True)).clamp_min(1e-30), where, ym)
-    assert len(xm) >= 2
-    _record(f"{family} out_f", L.regime, r1)
-    _record(f"{family} out_h", L.regime, r2)
-    return r1, r2
-
-
-def test_gemm_resid_ln_clusters():
-    """Clusters of 1..8 CTAs (N = 128 .. 1024), ragged last row of tiles, deep and shallow rings."""
-    _run_all(_cases(("RESID_LN",)), lambda c: _resid_ln(c.name, c.M, c.N, c.K, c.sms, "RESID_LN"))
-
-
-@pytest.mark.parametrize("name,M,N,K", kg.RESID_LN_PRODUCTION, ids=[p[0] for p in kg.RESID_LN_PRODUCTION])
-def test_resid_ln_at_production_shapes(name, M, N, K):
-    """attn.proj and mlp.fc2 as EPI_RESID_LN through mk_op_gemm at C2 (ViT-S, clusters of 3), C3 (ViT-B, 64 images,
-    clusters of 6) and ViT-L (one pair, clusters of 8)."""
-    r1, r2 = _resid_ln(name, M, N, K, _sms(), "RESID_LN production")
-    print(f"\n[{name}] RESID_LN max err/bound: out_f {r1:.3g}, out_h {r2:.3g}", end="")
-    ew.record("RESID_LN out_f", name, r1)
-    ew.record("RESID_LN out_h", name, r2)
-
-
-# ---------------------------------------------------------------------------------------------------------------
 # the matcher: EPI_LSE -> mk_op_matcher_reduce -> EPI_DUAL
 # ---------------------------------------------------------------------------------------------------------------
 def _matcher_case(c, lse_case):

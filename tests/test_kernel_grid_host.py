@@ -18,7 +18,6 @@ def test_dispatch_rule_at_known_shapes():
     assert L("STORE_H", 50001, 192, 5).bn == 64 and L("STORE_H", 50001, 192, 5).stages == 6
     # the one-tile-only epilogues never take the persistent kernel; EPI_DUAL through TMA stores is always shallow
     assert L("LN", 80000, 128, 4, groups=4).regime == "shallow"
-    assert L("RESID_LN", 64 * 1939, 768, 12).regime == "shallow"
     assert L("DUAL", 128, 128, 6, groups=1, out_tma=True).regime == "shallow"
     assert L("DUAL", 128, 128, 6, groups=1, out_tma=False).regime == "deep"
     # the cutovers
