@@ -195,6 +195,20 @@ class featureMatcher(_ParamTree):
         return mutual_matches(scores, min_conf)[0][0]
 
 
+REFERENCE_SAMPLED_MATCHES = 2048
+
+
+def check_sampled_matches(n):
+    """The drop-in solvers accept PROCRUSTES.NUM_SAMPLED_MATCHES = 2048 only.  The reference's estimate_pose_vectorized
+    reshapes its point tensors to 2048 samples per set (probabilisticProcrustes.py:271-272), so under any other value it
+    raises inside its try and returns the zero pose on every call; the CUDA solver (mk_solve_pose, mk_procrustes_solve)
+    would return real poses instead.  Such a configuration is rejected rather than silently generalised."""
+    if n != REFERENCE_SAMPLED_MATCHES:
+        raise ValueError(f"PROCRUSTES.NUM_SAMPLED_MATCHES must be {REFERENCE_SAMPLED_MATCHES}, got {n}: the reference "
+                         "reshapes its sampled sets to 2048 entries (probabilisticProcrustes.py:271-272) and returns the "
+                         "zero pose on every call under any other value")
+
+
 class e2eProbabilisticProcrustesSolver:
     """Test-time metric pose solver (reference probabilisticProcrustes.py:5-20, 183-348), CUDA-backed."""
 
@@ -207,6 +221,7 @@ class e2eProbabilisticProcrustesSolver:
         self.num_refinements = p.NUM_REFINEMENTS
         self.th_inlier = p.TH_INLIER
         self.th_soft_inlier = p.TH_SOFT_INLIER
+        check_sampled_matches(self.num_samples_matches)
         self._owner = owner
 
     def estimate_pose_vectorized(self, batch, return_inliers=False, outer_idx=None, inner_idx=None, seed=None):

@@ -17,10 +17,10 @@ import math
 import torch
 
 from . import _lib
-from .model import _inlier_list, _pose_views
+from .model import _inlier_list, _pose_views, check_sampled_matches
 
 # include/mickey_b200.h, mk_procrustes_solve's sizes
-MAX_SAMPLED, SAMPLED_STEP, MAX_GRID, INT_MAX = 2048, 256, 65535, 2 ** 31 - 1
+MAX_GRID, INT_MAX = 65535, 2 ** 31 - 1
 STATUS_ZERO = 1 | 2 | 4          # the status bits that give the zero result
 
 
@@ -42,9 +42,7 @@ class e2eProbabilisticProcrustesSolver:
             raise ValueError(f"PROCRUSTES.IT_MATCHES must be in [1, {MAX_GRID}], got {self.it_matches}")
         if not (self.it_RANSAC >= 1 and self.it_matches * self.it_RANSAC <= INT_MAX):
             raise ValueError(f"PROCRUSTES.IT_RANSAC must be >= 1 with IT_MATCHES * IT_RANSAC < 2^31, got {self.it_RANSAC}")
-        if not (SAMPLED_STEP <= self.num_samples_matches <= MAX_SAMPLED and self.num_samples_matches % SAMPLED_STEP == 0):
-            raise ValueError(f"PROCRUSTES.NUM_SAMPLED_MATCHES must be a multiple of {SAMPLED_STEP} up to {MAX_SAMPLED}, "
-                             f"got {self.num_samples_matches}")
+        check_sampled_matches(self.num_samples_matches)      # 2048 only: the reference's own limit, inside the kernels'
         if self.num_corr_3d_3d != 3:
             raise ValueError(f"PROCRUSTES.NUM_CORR_3D_3D must be 3, got {self.num_corr_3d_3d}")
         if self.num_refinements < 0:

@@ -346,7 +346,14 @@ def solve_pose(final_scores: Tensor, kps0: Tensor, depth0: Tensor, kps1: Tensor,
     outer_idx [B*IT_MATCHES, n_s] / inner_idx [B*IT_MATCHES*IT_RANSAC, 3]: when given they replace
     the two torch.multinomial draws (:231, :251) so that everything downstream is deterministic
     (this is how the CUDA solver is compared bit-for-bit in structure).  `trace`, when a dict, is
-    filled with the intermediate tensors (sampled indices, hypothesis scores, winner ...)."""
+    filled with the intermediate tensors (sampled indices, hypothesis scores, winner ...).
+
+    Where it departs from the reference: NUM_SAMPLED_MATCHES is taken from cfg for every shape.  The
+    reference hard-codes 2048 when it reshapes the point tensors (:271-272), so for any other value it
+    raises inside its try and returns the zero result; this restatement returns the pose the
+    algorithm defines.  It is the fp64 comparator of the CUDA solver's whole range (mk_procrustes_solve:
+    any multiple of 256 up to 2048); the drop-in solvers accept 2048 only (mickey_b200.model
+    check_sampled_matches)."""
     p = cfg["PROCRUSTES"]
     IM, IR, n_s, n_c = p["IT_MATCHES"], p["IT_RANSAC"], p["NUM_SAMPLED_MATCHES"], p["NUM_CORR_3D_3D"]
     B, N, _ = final_scores.shape

@@ -14,10 +14,14 @@ def _rot(axis, deg):
     return torch.eye(3, dtype=torch.float64) + math.sin(a) * Kx + (1 - math.cos(a)) * (Kx @ Kx)
 
 
-def planted_problem(n_side=(20, 16), batch=1, outlier_frac=0.4, seed=0, diag_weight=1.0, off_weight=1e-6):
+def planted_problem(n_side=(20, 16), batch=1, outlier_frac=0.4, seed=0, diag_weight=1.0, off_weight=1e-6, noise=0.0):
     """Keypoint i in image 0 corresponds to keypoint i in image 1: Y_i = R X_i + t exactly for the
     inlier fraction; the rest get a corrupted depth.  final_scores is diagonal-heavy so the sampler
-    picks (i, i) cells almost always.  Returns tensors shaped like the model's data dict."""
+    picks (i, i) cells almost always.  Returns tensors shaped like the model's data dict.
+
+    noise > 0 moves every Y_i by an isotropic Gaussian of that standard deviation (metres) before it is projected:
+    a hypothesis from three points is then off by more than the threshold far from them, and each refinement of the
+    solver adds the points its better fit brings inside (the inlier set grows over several refinements)."""
     g = torch.Generator().manual_seed(seed)
     h, w = n_side
     N = h * w
@@ -32,6 +36,8 @@ def planted_problem(n_side=(20, 16), batch=1, outlier_frac=0.4, seed=0, diag_wei
         d0 = torch.rand(N, generator=g, dtype=torch.float64) * 4 + 2
         X = d0 * (Kinv @ torch.cat([uv0, torch.ones(1, N, dtype=torch.float64)], 0))            # [3,N]
         Y = R @ X + t[:, None]
+        if noise > 0:
+            Y = Y + noise * torch.randn(3, N, generator=g, dtype=torch.float64)
         d1 = Y[2].clone()
         proj = K @ (Y / Y[2:3])
         uv1 = proj[:2]

@@ -71,14 +71,32 @@ def sampler_mode(N, pitch, aligned=True):
     return "SCALAR"
 
 
+def apply_overrides(cfg, overrides):
+    """overrides: {dotted config key: value}, e.g. {'MICKEY.KP_HEADS.USE_SOFTMAX': False}; every key must exist."""
+    for key, value in (overrides or {}).items():
+        node = cfg
+        *path, leaf = key.split(".")
+        for p in path:
+            node = node[p]
+        assert leaf in node, key
+        node[leaf] = value
+    return cfg
+
+
 class Run:
     """One compute_matches call on B synthetic pairs of H x W images and the geometry of its workspace.  A crop margin
-    (H or W not a multiple of 14) is filled with NaN: the patch gather must never read it."""
+    (H or W not a multiple of 14) is filled with NaN: the patch gather must never read it.  `overrides` changes the
+    configuration of mickey_cfg (apply_overrides): the head and matcher flags the stage checks follow."""
 
-    def __init__(self, name, variant, B, H, W, im, ir, regime=None):
+    def __init__(self, name, variant, B, H, W, im, ir, regime=None, overrides=None):
         self.name, self.B, self.H, self.W, self.im, self.ir = name, B, H, W, im, ir
         self.regime = regime                     # "persistent" / "one tile" / None: what the relaunched GEMMs must use
-        self.cfg = mickey_cfg(variant, im, ir)
+        self.cfg = apply_overrides(mickey_cfg(variant, im, ir), overrides)
+        m = self.cfg.MICKEY
+        self.use_softmax, self.depth_sigmoid = bool(m.KP_HEADS.USE_SOFTMAX), bool(m.KP_HEADS.USE_DEPTHSIGMOID)
+        self.max_depth, self.norm_dsc = float(m.KP_HEADS.MAX_DEPTH), bool(m.DSC_HEAD.NORM_DSC)
+        self.use_dustbin = bool(self.cfg.FEATURE_MATCHER.DUAL_SOFTMAX.USE_DUSTBIN)
+        self.temperature = float(self.cfg.FEATURE_MATCHER.DUAL_SOFTMAX.TEMPERATURE)
         model = MickeyRelativePose(self.cfg)
         model.load_state_dict(synthetic_state_dict(self.cfg, seed=3), strict=True)
         self.model = model.cuda().eval()
@@ -241,11 +259,16 @@ def check_conv(run, stage, A, cin, Wfull, groups, cout, three, got_of, *, a_col0
                 if pe_t is not None:
                     muts.append(ew.Mutation("PE row of the neighbouring position", (slice(vr, vr + 1), allr),
                                             (ref[vr:vr + 1] - pe_t[vr:vr + 1] + pe[pos[vr] + 1].double())))
+            if pe is not None and g not in pe_groups and r0 == 0:
+                # the PE on a group whose POS_ENCODING flag is off (a wrong aux_group_mask)
+                vr = int(run.valid[r0:r1].nonzero()[0])
+                muts.append(ew.Mutation(f"PE added to group {g}, whose flag is off", (slice(vr, vr + 1), allr),
+                                        ref[vr:vr + 1] + pe[pos[vr]].double()))
             planted += len(muts)
             where = ew.matrix_where(run.rows("padded"), tiles, row_offset=r0)
             where_g = ew.Where(lambda idx, g=g: (int(idx[0]), g, int(idx[1])), where.rows, tiles, r0)
             worst = max(worst, check(run, stage, f"{run.name} {stage} group {g}", got_of(g, r0, r1), ref, bound, where_g, muts))
-            assert not muts or g == groups - 1
+            assert not muts or g == groups - 1 or (pe is not None and g not in pe_groups)
     assert planted > 0, f"{run.name} {stage}: no mutation planted (R = {R})"
     return rec(run, stage, worst)
 
@@ -529,9 +552,17 @@ def head_outputs(run):
     depth = torch.cat([d["depth_kp0"], d["depth_kp1"]], 0)[:, 0]
     kps = torch.cat([d["kps0"], d["kps1"]], 0)
     score_raw = run.ws("score_raw", torch.float32, n_img, N)
-    muts = [ew.Mutation("token of the neighbouring image", (0, slice(9, 10)), a_d[1, 9:10])]
-    rec(run, "depth", check(run, "depth", f"{run.name} depth", depth, a_d, (b_d + U32 * a_d.abs()).clamp_min(1e-30),
-                            mutations=muts))
+    if run.depth_sigmoid:
+        # MAX_DEPTH sigma(a): the dot's error through sigma' <= sigma (1 - sigma); one expf (2 ulp), one add, one division
+        sg = torch.sigmoid(a_d)
+        d_ref = run.max_depth * sg
+        d_b = run.max_depth * sg * (1 - sg) * b_d + 8 * U32 * d_ref.abs() + 1e-37
+        muts = [ew.Mutation("token of the neighbouring image", (0, slice(9, 10)), d_ref[1, 9:10]),
+                ew.Mutation("MAX_DEPTH dropped from the depth sigmoid", (0, slice(9, 10)), sg[0, 9:10])]
+    else:
+        d_ref, d_b = a_d, b_d + U32 * a_d.abs()
+        muts = [ew.Mutation("token of the neighbouring image", (0, slice(9, 10)), a_d[1, 9:10])]
+    rec(run, "depth", check(run, "depth", f"{run.name} depth", depth, d_ref, d_b.clamp_min(1e-30), mutations=muts))
     rec(run, "score_raw", check(run, "score_raw", f"{run.name} score_raw", score_raw, a_s,
                                 (b_s + U32 * a_s.abs()).clamp_min(1e-30),
                                 mutations=[ew.Mutation("next token", (0, slice(9, 10)), a_s[0, 10:11])]))
@@ -543,32 +574,55 @@ def head_outputs(run):
     rec(run, "kps", check(run, "kps", f"{run.name} kps", kps, ref_k, bk,
                           mutations=[ew.Mutation("x and y swapped", (0, slice(0, 1), slice(kt, kt + 1)),
                                                  ref_k[0, 1:2, kt:kt + 1])]))
-    # score activation: spatial softmax (temperature 100) of the kernel's own raw map, 3-pixel border exactly zero
     r = score_raw.double()
-    mean = r.mean(-1, keepdim=True) + 1e-16
     inside = ((yy >= 3) & (yy < run.gh - 3) & (xx >= 3) & (xx < run.gw - 3))
-    arg = (r - mean) / 100
-    e = torch.where(inside, torch.exp(arg), torch.zeros_like(arg))
-    scr_ref = e / (e.sum(-1, keepdim=True) + 1e-16)
-    d_arg = (N * U32 * r.abs().mean(-1, keepdim=True) + U32 * mean.abs()) / 100 + 2 * U32 * arg.abs()
-    rel = 2 * (d_arg.amax(-1, keepdim=True) + 2.0 ** -22) + (N + 2) * U32
     scr = torch.cat([d["scr0"], d["scr1"]], 0)[:, 0]
-    bnd = torch.where(inside, scr_ref * rel, torch.zeros_like(scr_ref)).clamp_min(1e-30)
     c = int(inside.nonzero()[0])
     assert c == run.interior
-    rec(run, "score_softmax", check(run, "score_softmax", f"{run.name} scr", scr, scr_ref, bnd,
-                                    mutations=[ew.Mutation("next token", (0, slice(c, c + 1)), scr_ref[0, c + 1:c + 2])]))
-    assert float((scr.double().sum(-1) - 1).abs().max()) <= float(rel.max()) + N * U32
-    # descriptors: d / sqrt(sum d^2 + 1e-10), the squared norm, and the split operand of the matcher (bit-exact)
+    if run.use_softmax:
+        # score activation: spatial softmax (temperature 100) of the kernel's own raw map, 3-pixel border exactly zero
+        mean = r.mean(-1, keepdim=True) + 1e-16
+        arg = (r - mean) / 100
+        e = torch.where(inside, torch.exp(arg), torch.zeros_like(arg))
+        scr_ref = e / (e.sum(-1, keepdim=True) + 1e-16)
+        d_arg = (N * U32 * r.abs().mean(-1, keepdim=True) + U32 * mean.abs()) / 100 + 2 * U32 * arg.abs()
+        rel = 2 * (d_arg.amax(-1, keepdim=True) + 2.0 ** -22) + (N + 2) * U32
+        bnd = torch.where(inside, scr_ref * rel, torch.zeros_like(scr_ref)).clamp_min(1e-30)
+        rec(run, "score_softmax", check(run, "score_softmax", f"{run.name} scr", scr, scr_ref, bnd,
+                                        mutations=[ew.Mutation("next token", (0, slice(c, c + 1)), scr_ref[0, c + 1:c + 2])]))
+        assert float((scr.double().sum(-1) - 1).abs().max()) <= float(rel.max()) + N * U32
+    else:
+        # sigmoid(raw) inside the 3-cell border, exactly 0 outside: one expf (2 ulp) and one division of the kernel's own
+        # raw map (an expf that overflows gives 0 where sigmoid < 1e-37)
+        sg = torch.sigmoid(r)
+        scr_ref = torch.where(inside, sg, torch.zeros_like(sg))
+        bnd = torch.where(inside, 8 * U32 * scr_ref + 1e-37, torch.zeros_like(scr_ref)).clamp_min(1e-30)
+        rec(run, "score_sigmoid", check(run, "score_sigmoid", f"{run.name} scr", scr, scr_ref, bnd, mutations=[
+            ew.Mutation("next token", (0, slice(c, c + 1)), scr_ref[0, c + 1:c + 2]),
+            ew.Mutation("border dropped from the sigmoid score", (0, slice(0, 1)), sg[0, 0:1])]))
+    # descriptors: d / sqrt(sum d^2 + 1e-10) (or d itself without DSC_HEAD.NORM_DSC), the squared norm of what is stored,
+    # and the split operand of the matcher (bit-exact)
     ss = (Y4d * Y4d).sum(-1, keepdim=True)
-    dsc_ref = Y4d / torch.sqrt(ss + 1e-10)
-    rel_d = (129 / 2 + 4) * U32
+    normed = Y4d / torch.sqrt(ss + 1e-10)
     dsc = torch.cat([d["dsc0"], d["dsc1"]], 0).transpose(1, 2)
-    rec(run, "dsc", check(run, "dsc", f"{run.name} dsc", dsc, dsc_ref, (dsc_ref.abs() * rel_d).clamp_min(1e-30),
-                          mutations=[ew.Mutation("channels of the next token", (0, slice(3, 4)), dsc_ref[0, 4:5])]))
-    n2_ref = ss[..., 0] / (ss[..., 0] + 1e-10)
     nrm2 = run.ws("nrm2", torch.float32, n_img, N)
-    rec(run, "nrm2", check(run, "nrm2", f"{run.name} nrm2", nrm2, n2_ref, (129 + 2 * 69 + 4) * U32 * n2_ref.abs() + 1e-30))
+    if run.norm_dsc:
+        rel_d = (129 / 2 + 4) * U32
+        rec(run, "dsc", check(run, "dsc", f"{run.name} dsc", dsc, normed, (normed.abs() * rel_d).clamp_min(1e-30),
+                              mutations=[ew.Mutation("channels of the next token", (0, slice(3, 4)), normed[0, 4:5])]))
+        n2_ref = ss[..., 0] / (ss[..., 0] + 1e-10)
+        rec(run, "nrm2", check(run, "nrm2", f"{run.name} nrm2", nrm2, n2_ref, (129 + 2 * 69 + 4) * U32 * n2_ref.abs() + 1e-30))
+    else:
+        # desc_out_kernel stores Y4d as it is and its fp32 sum of squares (4 per lane, then a 5-step butterfly)
+        y32 = Y4d.float()
+        check_exact(run, "dsc", f"{run.name} dsc = Y4d", dsc, y32,
+                    mutations=[ew.Mutation("channels of the next token", (0, slice(3, 4)), y32[0, 4:5]),
+                               ew.Mutation("normalisation applied without NORM_DSC", (0, slice(3, 4)), normed[0, 3:4].float())])
+        rec(run, "dsc", 0.0)
+        n2_ref = ss[..., 0]
+        rec(run, "nrm2", check(run, "nrm2", f"{run.name} nrm2", nrm2, n2_ref, (129 * U32 * n2_ref).clamp_min(1e-30),
+                               mutations=[ew.Mutation("normalisation applied without NORM_DSC", (0, slice(3, 4)),
+                                                      (ss[0, 3:4, 0] / (ss[0, 3:4, 0] + 1e-10)))]))
     DSCX = run.ws("DSCX", torch.float16, n_img, N, 384)
     hi, lo = ew.split_hi_lo(dsc.contiguous())
     ref_x = torch.cat([torch.cat([hi[:B], lo[:B], hi[:B]], -1), torch.cat([hi[B:], hi[B:], lo[B:]], -1)], 0)
@@ -576,6 +630,23 @@ def head_outputs(run):
     check_exact(run, "dscx", f"{run.name} DSCX", DSCX, ref_x,
                 mutations=[ew.Mutation("hi and lo swapped in role 0", (slice(0, 1),), swapped)])
     rec(run, "dscx", 0.0)
+
+
+def _resolvable(v, bound, i=40):
+    """i when v[i + 1] differs from v[i] by more than twice i's bound, else the index where that margin is largest."""
+    if float((v[i + 1] - v[i]).abs()) > 2 * float(bound[i]):
+        return i
+    return int(((v[1:] - v[:-1]).abs() - 2 * bound[:-1]).argmax())
+
+
+def _swap_at(ref, bound, r, c):
+    """(r, c) when columns c..c+31 of row r + 1 differ from row r's by more than twice the bound somewhere, else the
+    row and 32-column chunk where that margin is largest (scores concentrated on a few cells at T = 1)."""
+    margin = (ref[:-1] - ref[1:]).abs() - 2 * bound[:-1]
+    if float(margin[r, c:c + 32].max()) > 0:
+        return r, c
+    i = int(margin.argmax())
+    return i // ref.shape[1], max(0, min(i % ref.shape[1] - 16, ref.shape[1] - 32))
 
 
 def matcher(run):
@@ -590,7 +661,16 @@ def matcher(run):
     # the 32-column chunk of the next row: row 500, columns 512..543 where the matrix holds them; on small grids the
     # first interior row (its final_scores row is zero outside the interior columns, which the chunk covers)
     sw_r, sw_c = (500, 512) if N > 600 else (run.interior, max(0, min(run.interior, N - 32)))
+    # engine.cu run_match: fixed-shift partials for unit-norm descriptors while 1 / T <= 25, true maxima otherwise; the
+    # bounds below hold in both modes
+    mode = "fixed-shift partials" if run.norm_dsc and inv_t <= 25.0 else "online-max partials"
+    tag = f"{run.name} ({mode}, {'with' if run.use_dustbin else 'without'} dustbin)"
     w_l = w_s = w_f = 0.0
+    dust_planted = 0
+
+    def lse2(v, dim):
+        return torch.logsumexp(v * math.log(2), dim) / math.log(2)
+
     for p in range(B):
         a, b = DSCX[p].double(), DSCX[B + p].double()
         d0, d1 = a[:, :128] + a[:, 128:256], b[:, :128] + b[:, 256:]
@@ -599,23 +679,39 @@ def matcher(run):
         x = S * k2
         dx = k2 * dS + 2 * U32 * x.abs()
         xd = torch.full((1, 1), dust, dtype=torch.float64, device=DEV)
-        lr = torch.logsumexp(torch.cat([x, xd.expand(N, 1)], 1) * math.log(2), 1) / math.log(2)
-        lc = torch.logsumexp(torch.cat([x, xd.expand(1, N)], 0) * math.log(2), 0) / math.log(2)
+        lr_d, lc_d = lse2(torch.cat([x, xd.expand(N, 1)], 1), 1), lse2(torch.cat([x, xd.expand(1, N)], 0), 0)
+        lr, lc = (lr_d, lc_d) if run.use_dustbin else (lse2(x, 1), lse2(x, 0))
         dlr = dx.amax(1) + ((N + 1) * U32 + 2.0 ** -22) / math.log(2) + 2.0 ** -22 * lr.abs()
         dlc = dx.amax(0) + ((N + 1) * U32 + 2.0 ** -22) / math.log(2) + 2.0 ** -22 * lc.abs()
-        muts = [ew.Mutation("lse of the next row", (slice(40, 41),), lr[41:42])]
-        w_l = max(w_l, check(run, "matcher_lse", f"{run.name} lse_r pair {p}", lse_r[p, :N], lr, dlr, mutations=muts))
-        w_l = max(w_l, check(run, "matcher_lse", f"{run.name} lse_c pair {p}", lse_c[p, :N], lc, dlc,
-                             mutations=[ew.Mutation("lse of the next column", (slice(40, 41),), lc[41:42])]))
+        # the row (column) 40 unless the next one's lse is within its bound (flat logits at T = 1): then the one most apart
+        rr, cc = _resolvable(lr, dlr), _resolvable(lc, dlc)
+        muts = [ew.Mutation("lse of the next row", (slice(rr, rr + 1),), lr[rr + 1:rr + 2])]
+        if not run.use_dustbin:
+            # the dustbin column included although USE_DUSTBIN is off, at the row where its share is largest; planted
+            # where that share is above four times the row's bound
+            i = int((lr_d - lr - 4 * dlr).argmax())
+            if float(lr_d[i] - lr[i]) > 4 * float(dlr[i]):
+                muts.append(ew.Mutation("dustbin included although USE_DUSTBIN is off", (slice(i, i + 1),), lr_d[i:i + 1]))
+                dust_planted += 1
+        w_l = max(w_l, check(run, "matcher_lse", f"{tag} lse_r pair {p}", lse_r[p, :N], lr, dlr, mutations=muts))
+        w_l = max(w_l, check(run, "matcher_lse", f"{tag} lse_c pair {p}", lse_c[p, :N], lc, dlc,
+                             mutations=[ew.Mutation("lse of the next column", (slice(cc, cc + 1),), lc[cc + 1:cc + 2])]))
         sc_ref = torch.exp2(2 * x - lr[:, None] - lc[None, :])
         rel = math.log(2) * (2 * dx + dlr[:, None] + dlc[None, :]) + 2.0 ** -22 + 4 * U32
         b_sc = sc_ref * rel + 2.0 ** -126
-        mut = [ew.row_chunk_swap(sc_ref, sw_r, sw_c)]
-        w_s = max(w_s, check(run, "matcher_scores", f"{run.name} scores pair {p}", d["scores"][p], sc_ref, b_sc, mutations=mut))
+        mut = [ew.row_chunk_swap(sc_ref, *_swap_at(sc_ref, b_sc, sw_r, sw_c))]
+        w_s = max(w_s, check(run, "matcher_scores", f"{tag} scores pair {p}", d["scores"][p], sc_ref, b_sc, mutations=mut))
         f_ref = sc_ref * scr[p][:, None] * scr[B + p][None, :]
-        w_f = max(w_f, check(run, "matcher_final_scores", f"{run.name} final_scores pair {p}", d["_final_scores_fused"][p],
-                             f_ref, f_ref * (rel + 3 * U32) + 2.0 ** -126, mutations=[ew.row_chunk_swap(f_ref, sw_r, sw_c)]))
+        b_f = f_ref * (rel + 3 * U32) + 2.0 ** -126
+        w_f = max(w_f, check(run, "matcher_final_scores", f"{tag} final_scores pair {p}", d["_final_scores_fused"][p],
+                             f_ref, b_f, mutations=[ew.row_chunk_swap(f_ref, *_swap_at(f_ref, b_f, sw_r, sw_c))]))
         del S, dS, x, dx, sc_ref, f_ref
+    # at T = 1 unit-norm descriptors bound every logit by 1, so the dustbin keeps a resolvable share of some row of each
+    # pair (DESIGN §6e); colder temperatures and raw descriptors can push it below every bound
+    assert run.use_dustbin or not (run.norm_dsc and run.temperature == 1.0) or dust_planted == B, \
+        f"{tag}: the dustbin's share is not resolvable"
+    if not run.use_dustbin:
+        print(f"\n[{run.name}] dustbin-included mutation planted in {dust_planted}/{B} pairs", end="")
     rec(run, "matcher_lse", w_l)
     rec(run, "matcher_scores", w_s)
     rec(run, "matcher_final_scores", w_f)
@@ -810,12 +906,12 @@ class Solved:
         self.N = self.fs.shape[-1]
 
 
-def band_all(fs_b, got, b, IM, seed, label):
-    """Band-check IM streams of pair b; returns (max n_diff, max n_band)."""
+def band_all(fs_b, got, b, IM, seed, label, n_s=N_S):
+    """Band-check IM streams of n_s cells of pair b; returns (max n_diff, max n_band)."""
     p = fs_b.reshape(-1).double()
     worst_diff = worst_band = 0
     for s, key in draws.outer_keys(p, seed, b, range(IM)):
-        r = draws.band_check(got[s], key, N_S)
+        r = draws.band_check(got[s], key, n_s)
         assert r["ok"], (label, b, s, r)
         worst_diff, worst_band = max(worst_diff, r["n_diff"]), max(worst_band, r["n_band"])
     return worst_diff, worst_band

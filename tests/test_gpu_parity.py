@@ -285,6 +285,10 @@ _FLAG_CASES = {
     "depth_sigmoid": {"MICKEY.KP_HEADS.USE_DEPTHSIGMOID": True},
     "no_dustbin": {"FEATURE_MATCHER.DUAL_SOFTMAX.USE_DUSTBIN": False},
     "no_pos_encoding": {"MICKEY.KP_HEADS.POS_ENCODING": False, "MICKEY.DSC_HEAD.POS_ENCODING": False},
+    # one PE flag each: rb3 conv2's aux_group_mask (engine.cu) is 0x7 / 0x8.  The element-wise stage checks start from
+    # the engine's intermediates and the later layers overwrite rb3's output in place, so a wrong mask shows only here.
+    "pos_encoding_kp_only": {"MICKEY.KP_HEADS.POS_ENCODING": True, "MICKEY.DSC_HEAD.POS_ENCODING": False},
+    "pos_encoding_dsc_only": {"MICKEY.KP_HEADS.POS_ENCODING": False, "MICKEY.DSC_HEAD.POS_ENCODING": True},
     "raw_descriptors": {"MICKEY.DSC_HEAD.NORM_DSC": False, "FEATURE_MATCHER.DUAL_SOFTMAX.TEMPERATURE": 20.0},
 }
 

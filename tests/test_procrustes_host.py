@@ -1,15 +1,23 @@
 """The handle-free pose solver without a GPU: the drop-in e2eProbabilisticProcrustesSolver's attributes and configuration
-checks, mk_procrustes_solve's host-side rejections (the pointers are never dereferenced), and
+checks (NUM_SAMPLED_MATCHES = 2048 only, as the live reference's zero result below 2048 shows), mk_procrustes_solve's
+host-side rejections (the pointers are never dereferenced), and
 use_cuda_modules(model, solver=True) on the recorded training-model tree and, when the reference tree is present, on the
 live MicKeyTrainingModel."""
 import ctypes as C
+import sys
 
 import pytest
 import torch
 
 from mickey_b200 import _lib
+from mickey_b200.config import mickey_cfg
+from mickey_b200.model import MickeyRelativePose
 from mickey_b200.procrustes import e2eProbabilisticProcrustesSolver
 from mickey_b200.training import use_cuda_modules
+from oracle import mickey_oracle as mo
+from oracle import ref_harness
+from tests import planted
+from tests.common import rotation_angle_deg
 from tests.golden import make_training_tree as mtt
 from tests.test_heads_host import model_from_tree, needs_reference
 
@@ -60,11 +68,60 @@ def test_unsupported_configurations_raise_at_construction(key, value):
         e2eProbabilisticProcrustesSolver(cfg)
 
 
-@pytest.mark.parametrize("S", [256, 512, 1792, 2048])
-def test_every_supported_set_size_is_accepted(S):
+@pytest.mark.parametrize("S", [256, 512, 1024, 1536, 1792])
+def test_set_sizes_the_reference_cannot_run_raise_at_construction(S):
+    """Multiples of 256 below 2048 are inside mk_procrustes_solve's range (tests/test_gpu_solver_params.py runs them),
+    but the reference returns the zero pose for every one of them (test_reference_returns_the_zero_pose_below_2048):
+    both drop-ins reject them, naming the reference's lines."""
     cfg = mtt.training_cfg()
     cfg.PROCRUSTES.NUM_SAMPLED_MATCHES = S
-    assert e2eProbabilisticProcrustesSolver(cfg).num_samples_matches == S
+    with pytest.raises(ValueError, match=r"NUM_SAMPLED_MATCHES must be 2048.*probabilisticProcrustes\.py:271-272"):
+        e2eProbabilisticProcrustesSolver(cfg)
+    icfg = mickey_cfg("vits")
+    icfg.PROCRUSTES.NUM_SAMPLED_MATCHES = S
+    with pytest.raises(ValueError, match=r"NUM_SAMPLED_MATCHES must be 2048.*probabilisticProcrustes\.py:271-272"):
+        MickeyRelativePose(icfg)
+    assert MickeyRelativePose(mickey_cfg("vits")).e2e_Procrustes.num_samples_matches == 2048
+
+
+def _reference_solver_class():
+    ref_harness._install_stubs()
+    saved = {k: v for k, v in sys.modules.items() if k == "lib" or k.startswith("lib.")}
+    for k in saved:
+        del sys.modules[k]
+    try:
+        with ref_harness._ref_on_path():
+            from lib.models.MicKey.modules.utils.probabilisticProcrustes import e2eProbabilisticProcrustesSolver as Ref
+    finally:
+        for k in [k for k in sys.modules if k == "lib" or k.startswith("lib.")]:
+            del sys.modules[k]
+        sys.modules.update(saved)
+    return Ref
+
+
+@needs_reference
+def test_reference_returns_the_zero_pose_below_2048():
+    """The live reference's estimate_pose_vectorized on a planted problem: a real pose at NUM_SAMPLED_MATCHES = 2048,
+    the zero result at 512 (its reshape to 2048 samples per set raises inside its try, :271-272), where the fp64
+    oracle, which stays general, returns the planted pose."""
+    Ref = _reference_solver_class()
+    p = planted.planted_problem((20, 16), batch=2, seed=5)
+    batch = {"final_scores": p["final_scores"], "kps0": p["kps0"], "kps1": p["kps1"], "depth_kp0": p["depth0"],
+             "depth_kp1": p["depth1"], "K_color0": p["K"], "K_color1": p["K"]}
+    cfg = mickey_cfg("vits", 2, 8)
+    torch.manual_seed(0)
+    R, t, inl = Ref(cfg).estimate_pose_vectorized(dict(batch))
+    assert float(R.abs().max()) > 0.5 and float(inl.abs().max()) > 0
+    cfg.PROCRUSTES.NUM_SAMPLED_MATCHES = 512
+    torch.manual_seed(0)
+    R, t, inl, lst = Ref(cfg).estimate_pose_vectorized(dict(batch), return_inliers=True)
+    assert torch.equal(R, torch.zeros(2, 3, 3)) and torch.equal(t, torch.zeros(2, 1, 3)) and torch.equal(inl, torch.zeros(2))
+    assert len(lst) == 2 and all(x.shape == (0, 5) for x in lst)
+    Ro, to, _ = mo.solve_pose(*(batch[k].double() for k in ("final_scores", "kps0", "depth_kp0", "kps1", "depth_kp1",
+                                                            "K_color0", "K_color1")), cfg,
+                              generator=torch.Generator().manual_seed(0))
+    assert float(rotation_angle_deg(Ro, p["R"].double()).max()) < 0.1            # fp32 keypoints: not exact
+    assert float((to.reshape(2, 3) - p["t"].double().reshape(2, 3)).abs().max()) < 1e-2
 
 
 # ---- mk_procrustes_solve's host checks ------------------------------------------------------------------------------
