@@ -277,6 +277,46 @@ int mk_loss_gradient(const int* sampled_idx_dev, const float* loss_value_dev, co
                      void* stream);
 long long mk_loss_gradient_ws_bytes(int B, int it_matches, int n_sample);
 
+/* ---- training loss, the differentiable tail (loss_class.py:140-152, 199-248) in CUDA: mickey_b200/loss.py's opt-in
+ * alternative to its autograd tail (MetricPoseLoss(cfg, cuda_tail=True)).  No handle.
+ *
+ * mk_loss_tail_forward: per hypothesis the weighted Procrustes on its inliers_final mask (fp64 Kabsch), the soft inlier
+ * score over all S entries, and the VCRE (loss_type 0) or POSE_ERR (loss_type 1) loss; per outer iteration the score
+ * softmax, with the null hypothesis (null_score = TH_OUTLIERS * S, null_loss = MAX_LOSS_SOFT/VALUE) when
+ * null_hypothesis != 0.  Inputs: sampled_idx_dev int32 [B*IM, S] and inliers_dev uint32 [B*IM*IR, S/32] as mk_loss_search
+ * writes them; kps0/kps1 [B,2,N], depth0/depth1 [B,1,N], K0/K1 (K_color), Kori0/Kori1 (Kori_color) fp32 [B,3,3], T_0to1
+ * fp32 [B,4,4] and grid_dev fp32 [MK_VCRE_POINTS,3] (mickey_b200.loss.vcre_grid()).  Out: loss_value_dev, loss_rot_dev,
+ * loss_trans_dev fp32 [B*IM]; status_dev int32[1] = MK_LOSS_TAIL_STATUS_NONFINITE when some hypothesis's R or t is not
+ * finite (the reference's zero result, :213-223).  The workspace keeps the forward's state for the backward: pass the
+ * same workspace, untouched, to mk_loss_tail_backward.
+ *
+ * mk_loss_tail_backward: from the upstream gradients of loss_value / loss_rot / loss_trans fp32 [B*IM] (the other
+ * arguments as given to the forward), writes every entry of dkps0/dkps1 fp32 [B,2,N] and ddepth0/ddepth1 fp32 [B,1,N]
+ * (0 at keypoints no set drew).  The rotation's backward needs no SVD (csrc/loss_tail.cu).  No float atomics: the
+ * gradients are the same bits on every run.
+ *
+ * Workspace: mk_loss_tail_ws_bytes(B, N, IM, IR, S) bytes (-1 for unsupported sizes).  Sizes: 1 <= B <= 65535, N >= 1 with
+ * N*N < 2^31, IM, IR >= 1 with B*IM*IR < 2^31, S a multiple of 32 up to 2048; inlier_3d_th finite and positive,
+ * score_temperature finite and non-zero.  Bad arguments (a NULL pointer, an unsupported size or parameter, a small
+ * workspace) return MK_ERR_INVALID with a message and launch nothing. */
+#define MK_LOSS_TAIL_STATUS_NONFINITE 1
+long long mk_loss_tail_ws_bytes(int B, int N, int it_matches, int it_ransac, int n_sample);
+int mk_loss_tail_forward(const int* sampled_idx_dev, const unsigned int* inliers_dev, const float* kps0_dev,
+                         const float* depth0_dev, const float* kps1_dev, const float* depth1_dev, const float* K0_dev,
+                         const float* K1_dev, const float* Kori0_dev, const float* Kori1_dev, const float* T_0to1_dev,
+                         const float* grid_dev, int B, int N, int it_matches, int it_ransac, int n_sample, int loss_type,
+                         int soft_clipping, int null_hypothesis, float inlier_3d_th, float score_temperature,
+                         float null_score, float null_loss, float* loss_value_dev, float* loss_rot_dev,
+                         float* loss_trans_dev, int* status_dev, void* ws_dev, long long ws_bytes, void* stream);
+int mk_loss_tail_backward(const int* sampled_idx_dev, const unsigned int* inliers_dev, const float* kps0_dev,
+                          const float* depth0_dev, const float* kps1_dev, const float* depth1_dev, const float* K0_dev,
+                          const float* K1_dev, const float* Kori0_dev, const float* Kori1_dev, const float* T_0to1_dev,
+                          const float* grid_dev, int B, int N, int it_matches, int it_ransac, int n_sample, int loss_type,
+                          int soft_clipping, int null_hypothesis, float inlier_3d_th, float score_temperature,
+                          const float* grad_loss_value_dev, const float* grad_loss_rot_dev,
+                          const float* grad_loss_trans_dev, float* dkps0_dev, float* dkps1_dev, float* ddepth0_dev,
+                          float* ddepth1_dev, void* ws_dev, long long ws_bytes, void* stream);
+
 /* ---- training: the dual-softmax matcher on the caller's descriptors and its backward (mickey_b200/dual_softmax.py wraps
  * both as a torch.autograd.Function).  Replaces dualSoftmax.forward (feature_matcher.py:64-83), kp_matrix_scores
  * (compute_correspondences.py:46-50) and scores * kp_scores (model.py:201), and autograd through them.  No handle.

@@ -136,6 +136,11 @@ EXPORTS = {
     "mk_loss_gradient": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
     "mk_loss_gradient_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int]),
+    "mk_loss_tail_ws_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mk_loss_tail_forward": (C.c_int, [C.c_void_p] * 12 + [C.c_int] * 8 + [C.c_float] * 4 + [C.c_void_p] * 5
+                             + [C.c_longlong, C.c_void_p]),
+    "mk_loss_tail_backward": (C.c_int, [C.c_void_p] * 12 + [C.c_int] * 8 + [C.c_float] * 2 + [C.c_void_p] * 8
+                              + [C.c_longlong, C.c_void_p]),
     "mk_dual_softmax_ws_bytes": (C.c_longlong, [C.c_int, C.c_int]),
     "mk_dual_softmax_backward_ws_bytes": (C.c_longlong, [C.c_int, C.c_int]),
     "mk_dual_softmax": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int,

@@ -70,4 +70,7 @@ long long loss_gradient_ws_bytes(int B, int IM, int S);
 int loss_gradient(const int* sampled, const float* loss_value, const float* baseline, const float* mask, int B, int N, int IM,
                   int S, float* grad, void* ws, long long ws_bytes, cudaStream_t st);
 
+// loss_tail.cu: the loss's differentiable tail, forward and backward (include/mickey_b200.h mk_loss_tail_forward)
+long long loss_tail_ws_bytes(int B, int N, int IM, int IR, int S);
+
 }  // namespace mk

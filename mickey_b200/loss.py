@@ -5,7 +5,8 @@ refinement search of every hypothesis (:163-196) and the dense REINFORCE gradien
 (:251-261, :299-316).  The small differentiable tail runs in autograd, exactly where the reference keeps gradients: one
 weighted Procrustes per hypothesis on its final inlier mask, the soft inlier score, the VCRE / POSE_ERR loss, the score
 softmax with the null hypothesis, the baseline and the curriculum top-K.  So `avg_loss.backward()` fills the kps / depth
-leaves of `outputs` through torch's own SVD backward, as in the reference.
+leaves of `outputs` through torch's own SVD backward, as in the reference.  MetricPoseLoss(cfg, cuda_tail=True) runs that
+tail in CUDA instead (csrc/loss_tail.cu, LossTail): the same arithmetic in fp64 and a closed-form backward with no SVD.
 
 Only `RANSAC_vectorized` is restated: the reference hard-codes `use_RANSAC_vectorized = True`.
 
@@ -154,6 +155,12 @@ class LossParams:
 def loss_search(fs, kps0, d0, kps1, d1, K0, K1, p: LossParams, seed: int, outer_idx=None, inner_idx=None):
     """mk_loss_search on a batch.  Returns (sampled int32 [B*IM, S], inner int32 [B*IM*IR, C], inliers_final {0,1} fp32
     [B*IM*IR, S], status int).  final_scores may be a view with contiguous rows and pairs N row pitches apart."""
+    sampled, inner, bits, status = _loss_search_bits(fs, kps0, d0, kps1, d1, K0, K1, p, seed, outer_idx, inner_idx)
+    return sampled, inner, unpack_mask(bits, p.n_sample), status
+
+
+def _loss_search_bits(fs, kps0, d0, kps1, d1, K0, K1, p: LossParams, seed: int, outer_idx=None, inner_idx=None):
+    """loss_search with inliers_final as the kernel writes it: int32 bit words [B*IM*IR, S/32]."""
     B, N = fs.shape[0], fs.shape[1]
     IM, IR, S, Cn = p.it_matches, p.it_ransac, p.n_sample, p.num_corr
     fs, pitch = _lib.pitched(fs)
@@ -176,7 +183,7 @@ def loss_search(fs, kps0, d0, kps1, d1, K0, K1, p: LossParams, seed: int, outer_
                                   _lib.ptr(K1), B, N, IM, IR, S, Cn, p.num_ref_steps, p.inlier_ref_th, seed, _lib.ptr(oi),
                                   _lib.ptr(ii), _lib.ptr(sampled), _lib.ptr(inner), _lib.ptr(bits), _lib.ptr(status),
                                   _lib.ptr(ws), ws.numel(), _lib.stream(dev)), "mk_loss_search")
-    return sampled, inner, unpack_mask(bits, S), int(status.item())
+    return sampled, inner, bits, int(status.item())
 
 
 def loss_gradient(sampled, loss_value, baseline, mask_topk, B, N, IM, S):
@@ -192,18 +199,71 @@ def loss_gradient(sampled, loss_value, baseline, mask_topk, B, N, IM, S):
     return grad
 
 
+class LossTail(torch.autograd.Function):
+    """The differentiable tail in CUDA (mk_loss_tail_forward / mk_loss_tail_backward): (loss_value, loss_rot, loss_trans)
+    fp32 [B*IM] and the status word int32 [1] from the search's drawn cells and inlier bit words, differentiable in the
+    kps / depth leaves.  The forward's saved state lives in a workspace allocated per call and kept on ctx only when a
+    backward can follow, so calls that interleave never share state and no_grad / inference_mode keep nothing."""
+
+    @staticmethod
+    def forward(ctx, kps0, depth0, kps1, depth1, sampled, bits, K0, K1, Kori0, Kori1, T, grid, p: LossParams, save: bool):
+        B, N = kps0.shape[0], kps0.shape[2]
+        IM, IR, S = p.it_matches, p.it_ransac, p.n_sample
+        dev = kps0.device
+        kps0, depth0, kps1, depth1 = (t.contiguous() for t in (kps0, depth0, kps1, depth1))
+        lib = _lib.load()
+        ws = _lib.workspace(lib.mk_loss_tail_ws_bytes(B, N, IM, IR, S), dev, "mk_loss_tail_ws_bytes")
+        out = torch.empty(3, B * IM, dtype=torch.float32, device=dev)
+        status = torch.empty(1, dtype=torch.int32, device=dev)
+        args = [_lib.ptr(t) for t in (sampled, bits, kps0, depth0, kps1, depth1, K0, K1, Kori0, Kori1, T, grid)]
+        args += [B, N, IM, IR, S, 0 if p.loss_type == "VCRE" else 1, int(p.soft_clipping), int(p.add_null_hypothesis),
+                 p.inlier_3d_th, p.score_temperature]
+        _lib.check(lib.mk_loss_tail_forward(*args, p.th_outliers * p.n_sample, p.max_loss_null, _lib.ptr(out[0]),
+                                            _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(status), _lib.ptr(ws), ws.numel(),
+                                            _lib.stream(dev)), "mk_loss_tail_forward")
+        ctx.mark_non_differentiable(status)
+        if save:
+            ctx.save_for_backward(kps0, depth0, kps1, depth1, sampled, bits, K0, K1, Kori0, Kori1, T, grid)
+            ctx.p, ctx.ws = p, ws
+        return out[0], out[1], out[2], status
+
+    @staticmethod
+    def backward(ctx, g_value, g_rot, g_trans, _g_status):
+        if not hasattr(ctx, "ws"):
+            raise RuntimeError("LossTail: the forward ran without saving its state (save=False)")
+        kps0, depth0, kps1, depth1, sampled, bits, K0, K1, Kori0, Kori1, T, grid = ctx.saved_tensors
+        p, ws = ctx.p, ctx.ws
+        B, N = kps0.shape[0], kps0.shape[2]
+        dev = kps0.device
+        g = [t.to(torch.float32).contiguous() for t in (g_value, g_rot, g_trans)]
+        dk0, dk1 = torch.empty_like(kps0), torch.empty_like(kps1)
+        dd0, dd1 = torch.empty_like(depth0), torch.empty_like(depth1)
+        lib = _lib.load()
+        args = [_lib.ptr(t) for t in (sampled, bits, kps0, depth0, kps1, depth1, K0, K1, Kori0, Kori1, T, grid)]
+        args += [B, N, p.it_matches, p.it_ransac, p.n_sample, 0 if p.loss_type == "VCRE" else 1, int(p.soft_clipping),
+                 int(p.add_null_hypothesis), p.inlier_3d_th, p.score_temperature]
+        _lib.check(lib.mk_loss_tail_backward(*args, *(_lib.ptr(t) for t in g), _lib.ptr(dk0), _lib.ptr(dk1), _lib.ptr(dd0),
+                                             _lib.ptr(dd1), _lib.ptr(ws), ws.numel(), _lib.stream(dev)),
+                   "mk_loss_tail_backward")
+        return dk0, dd0, dk1, dd1, None, None, None, None, None, None, None, None, None, None
+
+
 class MetricPoseLoss(torch.nn.Module):
     """Drop-in for the reference MetricPoseLoss(cfg): `forward(batch)` returns (avg_loss, outputs, [probs_grad],
     num_valid_h) with the reference's keys.  batch: final_scores [B, N, N], kps0/kps1 [B, 2, N], depth_kp0/depth_kp1
     [B, 1, N], K_color0/1 and Kori_color0/1 [B, 3, 3], T_0to1 [B, 4, 4], all on one CUDA device.  `topK` is settable
     (the training model raises it every epoch).  One seed is drawn from the torch RNG per call; `seed`, `outer_idx` and
     `inner_idx` override the draws (the parity tests inject the reference's).  After a call, `last_loss_value` [B*IM]
-    and `last_baseline` [B] hold the REINFORCE iteration losses and baselines (detached)."""
+    and `last_baseline` [B] hold the REINFORCE iteration losses and baselines (detached).
 
-    def __init__(self, cfg):
+    cuda_tail=True (also settable later) runs the differentiable tail in CUDA (LossTail) instead of autograd: the same
+    values to fp32 rounding, gradients through a closed-form, SVD-free backward, bit-identical from run to run."""
+
+    def __init__(self, cfg, cuda_tail: bool = False):
         super().__init__()
         self.p = LossParams(cfg)
         self.topK = self.p.topK
+        self.cuda_tail = bool(cuda_tail)
         self._grid = {}
 
     def _vcre_grid(self, dev):
@@ -229,7 +289,7 @@ class MetricPoseLoss(torch.nn.Module):
         K0, K1 = batch["K_color0"].float(), batch["K_color1"].float()
         if seed is None:
             seed = int(torch.randint(1, 2 ** 62, (1,)).item())     # follows torch.manual_seed like the reference
-        sampled, _, inl, status = loss_search(fs, kps0, depth0, kps1, depth1, K0, K1, p, seed, outer_idx, inner_idx)
+        sampled, _, bits, status = _loss_search_bits(fs, kps0, depth0, kps1, depth1, K0, K1, p, seed, outer_idx, inner_idx)
 
         outputs = {"kps0": kps0, "kps1": kps1, "depth0": depth0, "depth1": depth1}
         baseline = torch.zeros(B, device=dev)
@@ -238,7 +298,10 @@ class MetricPoseLoss(torch.nn.Module):
         loss_value = None
         num_valid_h = 0
         if not status & STATUS_SKIP:
-            tail = self._tail(batch, sampled, inl, kps0, depth0, kps1, depth1, K0, K1, Rgt, tgt, B, N)
+            if self.cuda_tail:
+                tail = self._cuda_tail(batch, sampled, bits, kps0, depth0, kps1, depth1, K0, K1)
+            else:
+                tail = self._tail(batch, sampled, unpack_mask(bits, S), kps0, depth0, kps1, depth1, K0, K1, Rgt, tgt, B, N)
             if tail is not None:
                 loss_value, loss_rot, loss_trans = tail
                 losses_rot = loss_rot.reshape(B, IM).sum(-1).unsqueeze(-1)
@@ -269,6 +332,21 @@ class MetricPoseLoss(torch.nn.Module):
         outputs["avg_t_errs"] = torch.mean(losses_trans)
         outputs["mask_topk"] = mask_topk
         return avg_loss, outputs, [gradients], num_valid_h
+
+    def _cuda_tail(self, batch, sampled, bits, kps0, depth0, kps1, depth1, K0, K1):
+        """_tail's values and gradients through LossTail, or None for the same invalid-pose early return."""
+        dev = kps0.device
+        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
+        leaves = (kps0, depth0, kps1, depth1)
+        if any(t.dtype != torch.float32 or t.device != dev for t in leaves):
+            raise ValueError("cuda_tail: kps0, kps1, depth_kp0 and depth_kp1 must be float32 tensors on one CUDA device")
+        save = torch.is_grad_enabled() and any(t.requires_grad for t in leaves)
+        loss_value, loss_rot, loss_trans, status = LossTail.apply(
+            *leaves, sampled, bits, f32(K0), f32(K1), f32(batch["Kori_color0"]), f32(batch["Kori_color1"]),
+            f32(batch["T_0to1"]), self._vcre_grid(dev), self.p, save)
+        if int(status.item()):
+            return None
+        return loss_value, loss_rot, loss_trans
 
     def _tail(self, batch, sampled, inl, kps0, depth0, kps1, depth1, K0, K1, Rgt, tgt, B, N):
         """:140-152 and :199-248 in autograd.  Returns (loss_value [B*IM], loss_rot [B*IM], loss_trans [B*IM]) or None

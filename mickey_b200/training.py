@@ -5,6 +5,7 @@
     model = MicKeyTrainingModel(cfg)
     use_cuda_modules(model)            # before trainer.fit, so that configure_optimizers collects the new modules' Parameters
     use_cuda_modules(model, solver=True)   # the same, and the validation's pose solver too
+    use_cuda_modules(model, cuda_tail=True)   # the same, and the loss's differentiable tail in CUDA
     trainer.fit(model, datamodule)
 
 See use_cuda_modules for what moves and what is kept.
@@ -55,7 +56,7 @@ def _transplant(new: nn.Module, old: nn.Module):
         m.training = flags.setdefault(n, flags[n.rpartition(".")[0]])
 
 
-def use_cuda_modules(model, solver: bool = False):
+def use_cuda_modules(model, solver: bool = False, cuda_tail: bool = False):
     """Replace, in place, the modules of the reference's MicKeyTrainingModel that have CUDA drop-ins, and return model:
 
         compute_matches.extractor.dinov2_vitl14      -> mickey_b200.dinov2.DinoVisionTransformer (the variant of its width)
@@ -71,7 +72,9 @@ def use_cuda_modules(model, solver: bool = False):
     curriculum state on_train_epoch_end moves, when the reference's loss has one (only with top-K or curriculum training).
     DINOV2.FLOAT16: False is rejected: the CUDA backbone runs in fp16 only.  model.e2e_Procrustes, the pose solver of the
     validation step and of the logging in backward_step, is replaced only with solver=True (it holds no parameters or
-    buffers, so the state dict is the same either way); by default it stays the reference's.
+    buffers, so the state dict is the same either way); by default it stays the reference's.  With cuda_tail=True the loss
+    runs its differentiable tail in CUDA (MetricPoseLoss(cfg, cuda_tail=True)); a loss that is already the drop-in gets the
+    flag set.  Without it the loss keeps the autograd tail (or whatever an earlier call chose).
 
     Call it before trainer.fit, so that configure_optimizers collects the new modules' Parameters.  Every replacement is
     built and checked before the model is touched: a configuration a drop-in rejects raises ValueError and leaves the
@@ -107,7 +110,7 @@ def use_cuda_modules(model, solver: bool = False):
         swaps.append((matcher, "matching_mat", new, old))
     old = model.loss_fn
     if not isinstance(old, MetricPoseLoss):
-        new = MetricPoseLoss(cfg)
+        new = MetricPoseLoss(cfg, cuda_tail=cuda_tail)
         if hasattr(old, "topK"):                 # the reference sets it only with top-K or curriculum training
             new.topK = old.topK
         swaps.append((model, "loss_fn", new, old))
@@ -122,4 +125,6 @@ def use_cuda_modules(model, solver: bool = False):
         setattr(parent, name, new)
     if procrustes is not None:
         model.e2e_Procrustes = procrustes
+    if cuda_tail:
+        model.loss_fn.cuda_tail = True
     return model
