@@ -57,7 +57,7 @@ int mk_finalize(mk_handle* h, int img_h, int img_w);
 
 long long mk_workspace_bytes(mk_handle* h, int n_pairs, int img_h, int img_w);
 /* Workspace of a call that extracts n_img images and matches / solves n_pairs pairs: (n, 0) for mk_extract_images,
- * (0, P) for mk_forward_pairs; (2P, P) equals mk_workspace_bytes(P). */
+ * (0, P) for mk_forward_pairs, (P, P) for mk_localize; (2P, P) equals mk_workspace_bytes(P). */
 long long mk_workspace_bytes_for(mk_handle* h, int n_img, int n_pairs, int img_h, int img_w);
 /* Byte offset of a named intermediate buffer inside the workspace (debugging / stage-wise tests; names and
  * layouts are listed in DESIGN.md §3: "X", "F", "CAT", "Y4d", ...). */
@@ -216,6 +216,34 @@ int mk_forward_pairs(mk_handle* h, const float* kps0_dev, const float* depth0_de
                      unsigned long long seed, float* kps_dev, float* depth_dev, float* scores_dev, float* kp_scores_dev,
                      float* final_scores_dev, long long nn_pitch, float* pose_dev, int* best_set_dev, float* inlier_mask_dev,
                      int* sampled_idx_out_dev, int* status_dev, void* ws_dev, long long ws_bytes, void* stream);
+
+/* ---- localization against cached references: replaces MickeyRelativePose.forward (compute_pose.py:20-37) for pairs
+ * (reference image ref_idx[p], query p) whose reference features mk_extract_images already computed.  Only the queries
+ * are extracted; pair p takes reference bank row ref_idx[p] in role 0 and query p in role 1.
+ * ref bank: kps [n_ref,2,N], depth [n_ref,1,N], scr [n_ref,1,N], dsc [n_ref,128,N] as mk_extract_images writes them, at the
+ * finalized geometry.  ref_idx_dev int32 [n_pairs] (device).  queries_dev fp32 [n_pairs,3,H,W] (mk_localize) or uint8
+ * [n_pairs,H,W,3] RGB (mk_localize_u8), as mk_forward / mk_forward_u8 read images.
+ * Out: kps_dev [2*n_pairs,2,N] and depth_dev [2*n_pairs,1,N] (required; reference rows first, as mk_forward_pairs);
+ * scr_dev [n_pairs,1,N] / dsc_dev [n_pairs,128,N]: the queries' scores and descriptors, each optional (NULL: not
+ * written); scores / kp_scores / final_scores / nn_pitch / pose / best_set / inlier_mask / sampled_idx as in mk_forward.
+ * Every output is bit-identical to mk_forward on the explicit pairs (reference image, query p), and to mk_forward_pairs
+ * on a query bank from mk_extract_images, with the same seed.  status_dev bit3 = an index outside [0, n_ref): nothing
+ * outside the bank is read and the batch gets the zero pose, as in mk_forward_pairs.  A NULL required pointer,
+ * n_pairs < 1, n_ref < 1 or an unfinalized handle returns MK_ERR_INVALID before anything is launched.  seed 0 continues
+ * the device-side sequence (capturable in a CUDA graph, replayed behind mk_set_seed).  Workspace:
+ * mk_workspace_bytes_for(n_pairs, n_pairs). */
+int mk_localize(mk_handle* h, const float* ref_kps_dev, const float* ref_depth_dev, const float* ref_scr_dev,
+                const float* ref_dsc_dev, int n_ref, const int* ref_idx_dev, const float* queries_dev, const float* K0_dev,
+                const float* K1_dev, int n_pairs, int img_h, int img_w, unsigned long long seed, float* kps_dev,
+                float* depth_dev, float* scr_dev, float* dsc_dev, float* scores_dev, float* kp_scores_dev,
+                float* final_scores_dev, long long nn_pitch, float* pose_dev, int* best_set_dev, float* inlier_mask_dev,
+                int* sampled_idx_out_dev, int* status_dev, void* ws_dev, long long ws_bytes, void* stream);
+int mk_localize_u8(mk_handle* h, const float* ref_kps_dev, const float* ref_depth_dev, const float* ref_scr_dev,
+                   const float* ref_dsc_dev, int n_ref, const int* ref_idx_dev, const unsigned char* queries_u8_dev,
+                   const float* K0_dev, const float* K1_dev, int n_pairs, int img_h, int img_w, unsigned long long seed,
+                   float* kps_dev, float* depth_dev, float* scr_dev, float* dsc_dev, float* scores_dev, float* kp_scores_dev,
+                   float* final_scores_dev, long long nn_pitch, float* pose_dev, int* best_set_dev, float* inlier_mask_dev,
+                   int* sampled_idx_out_dev, int* status_dev, void* ws_dev, long long ws_bytes, void* stream);
 
 /* ---- after the path: submission records (replaces the per-pair loop of submission.py:43-59)
  * pose_dev fp32 [n_pairs,13] as written by mk_forward / mk_solve_pose -> out_dev fp64 [n_pairs, 9] =

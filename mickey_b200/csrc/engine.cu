@@ -32,7 +32,7 @@ struct mk_handle {
 namespace {
 
 // n_img: images one call extracts; n_pairs: pairs it matches and solves.  mk_forward and its stages: (2P, P);
-// mk_extract_images: (n, 0); mk_forward_pairs: (0, P).
+// mk_extract_images: (n, 0); mk_forward_pairs: (0, P); mk_localize: (P, P), the P images being the role-1 queries.
 struct Geo {
   int H, W, gh, gw, N, T, h2, w2, per_img, n_img, n_pairs;
   long long M, Mp, R;
@@ -115,7 +115,8 @@ Workspace carve(void* base, const mk_config& c, const Geo& g) {
   Carver cv(base);
   const int n_pairs = g.n_pairs;
   const size_t D = c.embed_dim, R = g.R;
-  // the matcher's operands: written by the extraction (n_img images) or by the bank gather (2 * n_pairs role rows)
+  // the matcher's operands: written by the extraction (n_img images), by the bank gather (2 * n_pairs role rows) or by
+  // both (mk_localize: the gather fills the n_pairs role-0 rows, the extraction of n_img = n_pairs queries the role-1 rows)
   const size_t n_op = (size_t)std::max(g.n_img, 2 * g.n_pairs);
   const int* bd = c.block_dims;
   carve_backbone(cv, c, g, w);
@@ -245,8 +246,11 @@ int run_backbone(mk_handle* h, const void* images, int img_fmt, const Geo& g, Wo
   return MK_OK;
 }
 
+// role < 0: images [0, n_img/2) take role 0 in the matcher and the rest role 1 (mk_forward; mk_extract_images leaves
+// operands no matcher reads).  role 1: all n_img images are the queries of g.n_pairs = n_img pairs (mk_localize); their
+// operands and score copy go to the role-1 halves of DSCX and scr_copy.  dsc may be NULL (no fp32 descriptors).
 int run_extract(mk_handle* h, const void* images, int img_fmt, const Geo& g, float* kps, float* depth, float* scr,
-                float* dsc, Workspace& w, cudaStream_t st) {
+                float* dsc, Workspace& w, cudaStream_t st, int role = -1) {
   const mk_config& c = h->cfg;
   const int D = c.embed_dim;
   Lookup L{h};
@@ -364,8 +368,10 @@ int run_extract(mk_handle* h, const void* images, int img_fmt, const Geo& g, flo
                        w.score_raw, scr, g.n_img, g.gh, g.gw, c.depth_sigmoid, c.max_depth, (float)c.down_factor, c.use_softmax, st)); }
   if (!L.ok) return MK_ERR_MISSING_TENSOR;
   if (bd[3] != 64) { set_last_error("KP_HEADS.BLOCKS_DIM[3] must be 64"); return MK_ERR_UNSUPPORTED; }
-  MK_KERNEL("head.desc_out", desc_out(w.Y4d, dsc, w.DSCX, w.nrm2, g.n_img, g.gh, g.gw, c.norm_dsc, st));
-  MK_CUDA_CHECK(cudaMemcpyAsync(w.scr_copy, scr, (size_t)g.n_img * g.N * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  const size_t op_row = role == 1 ? (size_t)g.n_pairs * g.N : 0;       // first operand row this extraction writes
+  MK_KERNEL("head.desc_out", desc_out(w.Y4d, dsc, w.DSCX + op_row * 384, w.nrm2, g.n_img, g.gh, g.gw, c.norm_dsc, role, st));
+  if (scr != w.scr_copy + op_row)
+    MK_CUDA_CHECK(cudaMemcpyAsync(w.scr_copy + op_row, scr, (size_t)g.n_img * g.N * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return MK_OK;
 }
 
@@ -752,12 +758,67 @@ int mk_forward_pairs(mk_handle* h, const float* kps0, const float* depth0, const
   const Geo g = make_geo(0, n_pairs, h->geo_h, h->geo_w);
   cudaStream_t st = (cudaStream_t)stream;
   const BankView b0{kps0, depth0, scr0, dsc0, idx0, n0}, b1{kps1, depth1, scr1, dsc1, idx1, n1};
-  MK_KERNEL("pairs.gather", bank_gather(b0, b1, n_pairs, g.N, w.DSCX, kps, depth, w.scr_copy, st));
+  MK_KERNEL("pairs.gather", bank_gather(b0, b1, n_pairs, g.N, w.DSCX, kps, depth, w.scr_copy, 2, st));
   MK_TRY(run_match(h, n_pairs, g.N, scores, kp_scores, final_scores, nn_pitch, w, st));
   MK_TRY(run_solve_handle(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, g.N, seed, nullptr, nullptr, pose, best_set,
                           inl_mask, sampled_out, nullptr, status, w, st));
   MK_KERNEL("pairs.index_check", bank_index_check(b0, b1, n_pairs, pose, status, st));
   return MK_OK;
+}
+
+// Pair p = (reference ref_idx[p] in role 0, query p in role 1).  The role-0 gather and the queries' extraction write
+// disjoint halves of the operands, so the matcher and the solver then see exactly what mk_forward gives them.
+static int localize_any(mk_handle* h, const float* ref_kps, const float* ref_depth, const float* ref_scr, const float* ref_dsc,
+                        int n_ref, const int* ref_idx, const void* queries, int img_fmt, const float* K0, const float* K1,
+                        int n_pairs, int H, int W, unsigned long long seed, float* kps, float* depth, float* scr, float* dsc,
+                        float* scores, float* kp_scores, float* final_scores, long long nn_pitch, float* pose, int* best_set,
+                        float* inl_mask, int* sampled_out, int* status, void* ws, long long ws_bytes, void* stream) {
+  // every argument is checked before anything is launched
+  if (!h || n_pairs < 1 || n_ref < 1 || !ref_kps || !ref_depth || !ref_scr || !ref_dsc || !ref_idx || !queries || !K0 || !K1 ||
+      !kps || !depth || !final_scores || !pose) {
+    set_last_error("mk_localize: n_pairs %d and n_ref %d must be positive; the handle, the reference bank, ref_idx, the "
+                   "queries, K, kps, depth, final_scores and pose must be non-NULL", n_pairs, n_ref);
+    return MK_ERR_INVALID;
+  }
+  if ((scores == nullptr) != (kp_scores == nullptr)) {
+    set_last_error("mk_localize: scores and kp_scores are given together or both NULL (lean mode)");
+    return MK_ERR_INVALID;
+  }
+  Workspace w;
+  MK_TRY(check_ws(h, n_pairs, n_pairs, H, W, ws, ws_bytes, w));
+  const Geo g = make_geo(n_pairs, n_pairs, H, W);
+  long long pitch = nn_pitch;
+  MK_TRY(resolve_pitch(pitch, g.N, "mk_localize: nn_pitch"));
+  cudaStream_t st = (cudaStream_t)stream;
+  const BankView ref{ref_kps, ref_depth, ref_scr, ref_dsc, ref_idx, n_ref};
+  MK_KERNEL("localize.gather", bank_gather(ref, ref, n_pairs, g.N, w.DSCX, kps, depth, w.scr_copy, 1, st));
+  float* q_scr = scr ? scr : w.scr_copy + (size_t)n_pairs * g.N;     // without scr_dev the scores go straight to the operand
+  MK_TRY(run_extract(h, queries, img_fmt, g, kps + (size_t)n_pairs * 2 * g.N, depth + (size_t)n_pairs * g.N, q_scr, dsc, w, st, 1));
+  MK_TRY(run_match(h, n_pairs, g.N, scores, kp_scores, final_scores, nn_pitch, w, st));
+  MK_TRY(run_solve_handle(h, final_scores, nn_pitch, kps, depth, K0, K1, n_pairs, g.N, seed, nullptr, nullptr, pose, best_set,
+                          inl_mask, sampled_out, nullptr, status, w, st));
+  MK_KERNEL("localize.index_check", bank_index_check(ref, ref, n_pairs, pose, status, st));
+  return MK_OK;
+}
+
+int mk_localize(mk_handle* h, const float* ref_kps, const float* ref_depth, const float* ref_scr, const float* ref_dsc, int n_ref,
+                const int* ref_idx, const float* queries, const float* K0, const float* K1, int n_pairs, int H, int W,
+                unsigned long long seed, float* kps, float* depth, float* scr, float* dsc, float* scores, float* kp_scores,
+                float* final_scores, long long nn_pitch, float* pose, int* best_set, float* inl_mask, int* sampled_out,
+                int* status, void* ws, long long ws_bytes, void* stream) {
+  return localize_any(h, ref_kps, ref_depth, ref_scr, ref_dsc, n_ref, ref_idx, queries, 0, K0, K1, n_pairs, H, W, seed, kps, depth,
+                      scr, dsc, scores, kp_scores, final_scores, nn_pitch, pose, best_set, inl_mask, sampled_out, status, ws,
+                      ws_bytes, stream);
+}
+
+int mk_localize_u8(mk_handle* h, const float* ref_kps, const float* ref_depth, const float* ref_scr, const float* ref_dsc,
+                   int n_ref, const int* ref_idx, const unsigned char* queries, const float* K0, const float* K1, int n_pairs,
+                   int H, int W, unsigned long long seed, float* kps, float* depth, float* scr, float* dsc, float* scores,
+                   float* kp_scores, float* final_scores, long long nn_pitch, float* pose, int* best_set, float* inl_mask,
+                   int* sampled_out, int* status, void* ws, long long ws_bytes, void* stream) {
+  return localize_any(h, ref_kps, ref_depth, ref_scr, ref_dsc, n_ref, ref_idx, queries, 1, K0, K1, n_pairs, H, W, seed, kps, depth,
+                      scr, dsc, scores, kp_scores, final_scores, nn_pitch, pose, best_set, inl_mask, sampled_out, status, ws,
+                      ws_bytes, stream);
 }
 
 int mk_pose_to_submission(const float* pose, int n_pairs, double* out, void* stream) {

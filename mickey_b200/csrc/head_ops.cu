@@ -255,14 +255,16 @@ int kp_head_out(const float* y, const float* w_depth, const float* w_xy, const f
 // Descriptor output (mickey_extractor.py:246-249, extractor_utils.py:6-10): d / sqrt(sum d^2 + 1e-10).
 //   y fp32 [R, 128] -> dsc_cm fp32 [n_img, 128, N]   (the data-dict layout of the reference)
 //                   -> dsc_x  fp16 [n_img, N, 384]   (matcher operand: fp32 value split as hi + lo fp16;
-//                      role 0 images (img < n_img/2) store [hi | lo | hi], role 1 images [hi | hi | lo], so
+//                      role 0 images store [hi | lo | hi], role 1 images [hi | hi | lo], so
 //                      that one K=384 fp16 GEMM yields hi0.hi1 + lo0.hi1 + hi0.lo1 ~ fp32 dot product)
 //                   -> nrm2 fp32 [n_img, N]  squared norm of the stored descriptor
+// role < 0: an image's role is its half of the batch (img < n_img/2: role 0), as mk_forward extracts image0 then image1;
+// role 0 / 1: every image takes that role (mk_localize extracts only queries).  dsc_cm == NULL: no fp32 copy.
 // one warp per valid token, 4 channels per lane.
 // ------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 desc_out_kernel(const float* __restrict__ y, float* __restrict__ dsc_cm, __half* __restrict__ dsc_x,
-                float* __restrict__ nrm2, int n_img, int gh, int gw, int normalize) {
+                float* __restrict__ nrm2, int n_img, int gh, int gw, int normalize, int role) {
   pdl_wait();        // launched with programmatic stream serialization: predecessors are complete past this point
   pdl_trigger();
   const int tok = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -285,11 +287,11 @@ desc_out_kernel(const float* __restrict__ y, float* __restrict__ dsc_cm, __half*
   __half hi[4], lo[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    dsc_cm[((long long)im * 128 + lane * 4 + i) * N + n] = vals[i];
+    if (dsc_cm) dsc_cm[((long long)im * 128 + lane * 4 + i) * N + n] = vals[i];
     hi[i] = __float2half_rn(vals[i]);
     lo[i] = __float2half_rn(vals[i] - __half2float(hi[i]));
   }
-  const bool role1 = im >= n_img / 2;
+  const bool role1 = role < 0 ? im >= n_img / 2 : role == 1;
   __half* dst = dsc_x + ((long long)im * N + n) * 384 + lane * 4;
   uint2 uh, ul;
   uh.x = (uint32_t)__half_as_ushort(hi[0]) | ((uint32_t)__half_as_ushort(hi[1]) << 16);
@@ -301,16 +303,18 @@ desc_out_kernel(const float* __restrict__ y, float* __restrict__ dsc_cm, __half*
   *reinterpret_cast<uint2*>(dst + 256) = role1 ? ul : uh;
 }
 
-int desc_out(const float* y, float* dsc_cm, void* dsc_x, float* nrm2, int n_img, int gh, int gw, int normalize,
+int desc_out(const float* y, float* dsc_cm, void* dsc_x, float* nrm2, int n_img, int gh, int gw, int normalize, int role,
              cudaStream_t s) {
-  MK_CUDA_CHECK(launch_k(desc_out_kernel, dim3(ceil_div(n_img * gh * gw, 8)), dim3(256), 0, s, y, dsc_cm, (__half*)dsc_x, nrm2, n_img, gh, gw, normalize));
+  MK_CUDA_CHECK(launch_k(desc_out_kernel, dim3(ceil_div(n_img * gh * gw, 8)), dim3(256), 0, s, y, dsc_cm, (__half*)dsc_x, nrm2, n_img, gh, gw,
+                         normalize, role));
   MK_CUDA_CHECK(cudaGetLastError());
   return MK_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Feature-bank gather (mk_forward_pairs): the per-pair operands of the matcher and the solver, taken from two banks of
-// extracted images.  Block (x, p, r): tokens [32x, 32x + 32) of pair p in role r; its image is idx_r[p] of bank r.
+// Feature-bank gather (mk_forward_pairs, mk_localize): the per-pair operands of the matcher and the solver, taken from
+// banks of extracted images.  Block (x, p, r): tokens [32x, 32x + 32) of pair p in role r; its image is idx_r[p] of bank
+// r.  mk_forward_pairs launches both roles; mk_localize only role 0 (grid z = 1), since it extracts the role-1 queries.
 //   dsc  fp32 [n, 128, N] channel-major -> dsc_x fp16 [(r*P + p)*N + tok, 384], split exactly as desc_out_kernel does
 //   kps [n,2,N], depth [n,1,N], scr [n,1,N] -> kps_out [2P,2,N], depth_out [2P,1,N], scr_out [2P,N]  (role-0 rows first)
 // The descriptor tile is transposed through shared memory: each warp reads 128-byte runs of 32 tokens of one channel and
@@ -361,8 +365,8 @@ bank_gather_kernel(BankView b0, BankView b1, int P, int N, __half* __restrict__ 
 }
 
 int bank_gather(const BankView& b0, const BankView& b1, int P, int N, void* dsc_x, float* kps_out, float* depth_out, float* scr_out,
-                cudaStream_t s) {
-  MK_CUDA_CHECK(launch_k(bank_gather_kernel, dim3(ceil_div(N, 32), P, 2), dim3(256), 0, s, b0, b1, P, N, (__half*)dsc_x, kps_out,
+                int n_roles, cudaStream_t s) {
+  MK_CUDA_CHECK(launch_k(bank_gather_kernel, dim3(ceil_div(N, 32), P, n_roles), dim3(256), 0, s, b0, b1, P, N, (__half*)dsc_x, kps_out,
                          depth_out, scr_out));
   MK_CUDA_CHECK(cudaGetLastError());
   return MK_OK;

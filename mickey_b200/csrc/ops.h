@@ -25,13 +25,16 @@ int linattn_msg(const float* qkv, const float* kv, void* msg, int n_img, int G, 
 int kp_head_out(const float* y, const float* w_depth, const float* w_xy, const float* w_score, float* depth, float* kps,
                 float* score_raw, float* scr, int n_img, int gh, int gw, int depth_sigmoid, float max_depth,
                 float down_factor, int use_softmax, cudaStream_t s);
-int desc_out(const float* y, float* dsc_cm, void* dsc_x, float* nrm2, int n_img, int gh, int gw, int normalize, cudaStream_t s);
+// role < 0: the first half of the images are role 0, the second half role 1; role 0 / 1: all images.  dsc_cm may be NULL.
+int desc_out(const float* y, float* dsc_cm, void* dsc_x, float* nrm2, int n_img, int gh, int gw, int normalize, int role,
+             cudaStream_t s);
 int matcher_lse_reduce(const void* part_row, const void* part_col, const float* dustbin, int B, int N, int part_ld, float* lse_r,
                        float* lse_c, cudaStream_t s);
 // one bank of extracted images (kps [n,2,N], depth [n,1,N], scr [n,1,N], dsc [n,128,N]) and the image index of every pair
 struct BankView { const float *kps, *depth, *scr, *dsc; const int* idx; int count; };
+// n_roles 2: both roles (b0 then b1); 1: role 0 only (its rows of dsc_x, kps_out, depth_out, scr_out)
 int bank_gather(const BankView& b0, const BankView& b1, int P, int N, void* dsc_x, float* kps_out, float* depth_out, float* scr_out,
-                cudaStream_t s);
+                int n_roles, cudaStream_t s);
 int bank_index_check(const BankView& b0, const BankView& b1, int P, float* pose, int* status, cudaStream_t s);
 
 // matches.cu: featureMatcher.get_matches_list, batched (include/mickey_b200.h mk_mutual_matches)

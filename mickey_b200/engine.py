@@ -11,6 +11,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import math
+import weakref
 from typing import Dict, Optional
 
 import torch
@@ -220,6 +221,14 @@ def sine_table_padded(gh: int, gw: int, d_model: int = 128) -> torch.Tensor:
     return out.reshape(-1, d_model).contiguous()
 
 
+def _version_of(t):
+    """t's version counter, which in-place torch ops on t or its views advance; None for inference tensors (no counter)."""
+    try:
+        return t._version
+    except RuntimeError:
+        return None
+
+
 # ---------------------------------------------------------------------------------------------------------
 class Engine(_lib.Handle):
     """One C handle + packed weights + workspace for a fixed (cfg, device)."""
@@ -248,6 +257,7 @@ class Engine(_lib.Handle):
         self._graphs, self._slot = {}, {}
         self._copy_stream = None
         self._pairs_ws = None
+        self._loc_ws = None
         # set when the engine takes new blocks on the caller's stream (weights, tables, workspace, buffer sets): that stream
         # may still have work queued on those blocks (writes of the weights and tables, or pending kernels of tensors freed
         # there), so the streams that use them next wait on it once
@@ -268,6 +278,7 @@ class Engine(_lib.Handle):
         yield from self.packed.values()
         yield self.ws
         yield self._pairs_ws
+        yield self._loc_ws
         for gs in self._geo_state.values():
             yield from (gs[n] for n in ("patch.posb", "patch.clspos", "head.pe", "ws"))
         for ent in self._graphs.values():
@@ -553,22 +564,33 @@ class Engine(_lib.Handle):
             raise _lib.MickeyB200Error(f"image0 {tuple(image0.shape)} and image1 {tuple(image1.shape)} must have the same shape: "
                                        "both images of a batch go through one extraction call")
         self._ws_for(B, H, W)
+        ent = self._buffer_set((B, H, W), (bool(u8), bool(lean)), self.ws, lambda: self._static_buffers(B, H, W, u8, lean))
+        st = ent["st"]
+        return self._issue(ent, (image0, image1, K0, K1), (st["images"][:B], st["images"][B:], st["K0"], st["K1"]),
+                           lambda s: self._call_forward(st, B, H, W, s), seed, use_graph)
+
+    def _buffer_set(self, shape, fmt, ws, make):
+        """The static buffer set of a forward() / localize() call of shape (n, H, W) and format fmt: two sets alternate per
+        (shape, fmt); a set (with its graph) is rebuilt when the workspace ws it was captured with has moved."""
         if self._copy_stream is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
-        fmt = (bool(u8), bool(lean))
-        slot = self._slot.get((B, H, W, fmt), 0)
-        self._slot[(B, H, W, fmt)] = slot ^ 1
-        key = (B, H, W, slot, fmt)
+        slot = self._slot.get((*shape, fmt), 0)
+        self._slot[(*shape, fmt)] = slot ^ 1
+        key = (*shape, slot, fmt)
         ent = self._graphs.get(key)
-        if ent is None or ent["ws_ptr"] != self.ws.data_ptr():
-            ent = {"st": {k: self._own(t) for k, t in self._static_buffers(B, H, W, u8, lean).items()}, "graph": None,
-                   "launches": 0, "ws_ptr": self.ws.data_ptr(), "calls": 0, "done": None, "readers": set()}
+        if ent is None or ent["ws_ptr"] != ws.data_ptr():
+            ent = {"st": {k: self._own(t) for k, t in make().items()}, "graph": None,
+                   "launches": 0, "ws_ptr": ws.data_ptr(), "calls": 0, "done": None, "readers": set()}
             self._graphs[key] = ent
             self._caller_pending = True
+        return ent
+
+    def _issue(self, ent, ops, dst, call, seed, use_graph, before=None):
+        """Issue one call of buffer set ent: copy the inputs ops into dst, run before() (on the engine's stream, after
+        those copies), then call(seed) eagerly or from the set's graph.  Returns the set's static tensors."""
         st = ent["st"]
         caller = torch.cuda.current_stream()
         main = self.stream if self.stream is not None else caller
-        ops = (image0, image1, K0, K1)
         fresh, self._caller_pending = self._caller_pending, False
         if self.stream is not None:
             if ent.get("released") is not None:
@@ -584,7 +606,7 @@ class Engine(_lib.Handle):
             if fresh or (on_device and not self.assume_inputs_ready):
                 main.wait_stream(caller)                # device inputs may still be being produced on the caller's stream
         with torch.cuda.stream(main):
-            self._forward_on(main, ent, st, ops, B, H, W, seed, use_graph, caller if fresh else None)
+            self._forward_on(main, ent, dst, ops, call, seed, use_graph, caller if fresh else None, before)
         if self.stream is not None:
             caller.wait_event(ent["done"])              # outputs are safe to consume on the caller's stream
         self._last_ent = ent
@@ -599,8 +621,7 @@ class Engine(_lib.Handle):
             ev.record()
             self._last_ent["released"] = ev
 
-    def _forward_on(self, main, ent, st, ops, B, H, W, seed, use_graph, caller_pending):
-        dst = (st["images"][:B], st["images"][B:], st["K0"], st["K1"])
+    def _forward_on(self, main, ent, dst, ops, call, seed, use_graph, caller_pending, before):
         if any(t.device.type == "cpu" for t in ops):
             cs = self._copy_stream
             if caller_pending is not None:
@@ -615,14 +636,16 @@ class Engine(_lib.Handle):
         for d, s in zip(dst, ops):                      # device operands: in order behind the caller's stream (see forward)
             if s.device.type != "cpu":
                 d.copy_(s, non_blocking=True)
+        if before is not None:
+            before()
         seed = self._forward_seed(seed)
         if not use_graph:
-            self._call_forward(st, B, H, W, seed)
+            call(seed)
         elif ent["graph"] is None and ent["calls"] == 0:
             # first call of this buffer set runs eagerly (one-time lazy initialisation inside the library:
             # function attributes, TMA descriptors); the second call is captured, later calls replay
             l0 = self.launch_count
-            self._call_forward(st, B, H, W, seed)
+            call(seed)
             ent["launches"] = self.launch_count - l0
             ent["calls"] = 1
         else:
@@ -630,7 +653,7 @@ class Engine(_lib.Handle):
             if ent["graph"] is None:
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    self._call_forward(st, B, H, W, 0)      # seed 0 = continue the device-side sequence
+                    call(0)                                 # seed 0 = continue the device-side sequence
                 ent["graph"] = g
             ent["graph"].replay()
             self.graph_replays = getattr(self, "graph_replays", 0) + 1
@@ -638,6 +661,82 @@ class Engine(_lib.Handle):
         if ent["done"] is None:
             ent["done"] = torch.cuda.Event()
         ent["done"].record(main)
+
+    # -- localization against cached references: only the queries are extracted (mk_localize) ---------------------------
+    REF_KEYS = ("ref.kps", "ref.depth", "ref.scr", "ref.dsc")
+
+    def _localize_ws(self, P, H, W):
+        """Workspace of localize(), apart from forward()'s and the feature banks': localize()'s buffer sets and graphs hold
+        its address.  It grows to the largest call seen; a set captured on an outgrown workspace is rebuilt."""
+        nbytes = self.lib.mk_workspace_bytes_for(self.h, P, P, H, W)
+        if self._loc_ws is None or self._loc_ws.numel() < nbytes:
+            self._loc_ws = self._own(_lib.workspace(nbytes, self.device, "mk_workspace_bytes_for"))
+            self._caller_pending = True
+        return self._loc_ws
+
+    def _localize_buffers(self, P, H, W, n_ref, u8, lean):
+        dev, D, N = self.device, self.mkcfg.desc_dim, (H // PATCH) * (W // PATCH)
+        queries = torch.empty(P, H, W, 3, dtype=torch.uint8, device=dev) if u8 else torch.empty(P, 3, H, W, device=dev)
+        ref = (torch.empty(n_ref, 2, N, device=dev), torch.empty(n_ref, 1, N, device=dev), torch.empty(n_ref, 1, N, device=dev),
+               torch.empty(n_ref, D, N, device=dev))
+        out = self._outputs(2 * P, P, N, lean, scr_dsc=False)
+        return {"queries": queries, "ref_idx": torch.empty(P, dtype=torch.int32, device=dev),
+                "K0": torch.empty(P, 3, 3, device=dev), "K1": torch.empty(P, 3, 3, device=dev), **dict(zip(self.REF_KEYS, ref)),
+                "kps": out.pop("kps"), "depth": out.pop("depth"), "scr": torch.empty(P, 1, N, device=dev),
+                "dsc": torch.empty(P, D, N, device=dev), **out}
+
+    def _call_localize(self, st, ws, n_ref, P, H, W, seed):
+        fn = self.lib.mk_localize_u8 if st["queries"].dtype == torch.uint8 else self.lib.mk_localize
+        p = _lib.ptr
+        _lib.check(fn(self.h, *(p(st[k]) for k in self.REF_KEYS), n_ref, p(st["ref_idx"]), p(st["queries"]), p(st["K0"]),
+                      p(st["K1"]), P, H, W, C.c_ulonglong(seed), *self._output_args(st), p(ws), ws.numel(), _lib.stream()),
+                   "mk_localize")
+
+    def localize(self, ref_bank, ref_idx, queries, K0, K1, seed: int, use_graph: bool = True, lean: bool = False):
+        """Pose P queries against cached references in one C call (mk_localize): pair p = (reference ref_idx[p], query p).
+
+        ref_bank = (kps, depth, scr, dsc) of n_ref references as extract_images returns them (fp32, contiguous, on the
+        engine's device), extracted at the queries' token grid; ref_idx int [P] in [0, n_ref) (host or device); queries
+        fp32 [P, 3, H, W] or uint8 [P, H, W, 3] RGB, K0 / K1 [P, 3, 3], host (pinned) or device, as forward() takes them.
+        Returns the static tensors of this call's buffer set, with forward()'s lifetime rules: kps [2P,2,N] and depth
+        [2P,1,N] (reference rows first), the queries' scr [P,1,N] and dsc [P,128,N], scores / kp_scores (None when lean),
+        final_scores, pose, best_set, inlier_mask, sampled_idx, status.
+
+        A captured graph must not read the caller's tensors, which may be freed or changed before a replay: each buffer set
+        holds a copy of the reference bank (its reference slot), refreshed on the engine's stream whenever the bank's
+        tensors are not the objects last copied (held by weak reference, so a new tensor at a freed one's address is
+        still new) or their version counters moved (an in-place torch op on them or a view of them).  Writes that bypass
+        the version counter (through .data or a raw pointer) are not seen: pass new tensors after such writes."""
+        u8 = queries.dtype == torch.uint8
+        if u8:
+            if queries.dim() != 4 or queries.shape[-1] != 3:
+                raise _lib.MickeyB200Error("uint8 queries must be [P, H, W, 3] (HWC, RGB)")
+            P, H, W = queries.shape[:3]
+        else:
+            P, H, W = queries.shape[0], queries.shape[-2], queries.shape[-1]
+        n_ref = ref_bank[0].shape[0]
+        self._use_geometry(H, W)
+        ws = self._localize_ws(P, H, W)
+        ent = self._buffer_set((P, H, W), ("localize", bool(u8), bool(lean), n_ref), ws,
+                               lambda: self._localize_buffers(P, H, W, n_ref, u8, lean))
+        st = ent["st"]
+        src = tuple(ref_bank)
+        seen = ent.get("ref_src")
+        stale = seen is None or any(r() is not t or v is None or v != _version_of(t) for (r, v), t in zip(seen, src))
+        if stale:
+            # the slot's copies read the caller's tensors: like new engine blocks, they wait for the caller's stream
+            self._caller_pending = True
+
+        def refresh():
+            if stale:
+                for k, t in zip(self.REF_KEYS, src):
+                    st[k].copy_(t, non_blocking=True)
+                    if self.stream is not None:
+                        t.record_stream(self.stream)        # the caller may drop t before this copy has run
+                ent["ref_src"] = tuple((weakref.ref(t), _version_of(t)) for t in src)
+
+        return self._issue(ent, (queries, ref_idx, K0, K1), (st["queries"], st["ref_idx"], st["K0"], st["K1"]),
+                           lambda s: self._call_localize(st, ws, n_ref, P, H, W, s), seed, use_graph, before=refresh)
 
     def solve(self, final_scores, kps, depth, K0, K1, seed: int, outer_idx=None, inner_idx=None):
         """kps [2B,2,N], depth [2B,1,N] as produced by extract (image0 rows first).  final_scores [B,N,N] may be a padded

@@ -94,17 +94,59 @@ def validate_pairs(feats0: MickeyFeatures, idx0, feats1: MickeyFeatures, idx1) -
     if feats0.grid != feats1.grid:
         raise MickeyB200Error(f"banks of token grids {feats0.grid} and {feats1.grid}: both must come from one geometry")
     for b in (feats0, feats1):
-        if tuple(b.grid) != (b.image_size[0] // PATCH, b.image_size[1] // PATCH):
-            raise MickeyB200Error(f"bank grid {b.grid} is not the token grid of its image size {b.image_size}")
-        N = b.grid[0] * b.grid[1]
-        if tuple(b.kps.shape[1:]) != (2, N) or tuple(b.dsc.shape[2:]) != (N,) or b.depth.shape[-1] != N or b.scr.shape[-1] != N:
-            raise MickeyB200Error(f"bank tensors {tuple(b.kps.shape)} / {tuple(b.dsc.shape)} do not match its grid {b.grid}")
-        if any(t.shape[0] != len(b) for t in b.tensors()):
-            raise MickeyB200Error("bank tensors hold different image counts")
+        _check_bank(b)
     devs = {t.device for b in (feats0, feats1) for t in b.tensors()}
     if len(devs) != 1:
         raise MickeyB200Error(f"bank tensors on several devices: {sorted(map(str, devs))}")
     return i0, i1
+
+
+def _check_bank(b: MickeyFeatures):
+    if tuple(b.grid) != (b.image_size[0] // PATCH, b.image_size[1] // PATCH):
+        raise MickeyB200Error(f"bank grid {b.grid} is not the token grid of its image size {b.image_size}")
+    N = b.grid[0] * b.grid[1]
+    if tuple(b.kps.shape[1:]) != (2, N) or tuple(b.dsc.shape[2:]) != (N,) or b.depth.shape[-1] != N or b.scr.shape[-1] != N:
+        raise MickeyB200Error(f"bank tensors {tuple(b.kps.shape)} / {tuple(b.dsc.shape)} do not match its grid {b.grid}")
+    if any(t.shape[0] != len(b) for t in b.tensors()):
+        raise MickeyB200Error("bank tensors hold different image counts")
+
+
+def validate_localize(reference: MickeyFeatures, ref_idx, queries, K_color0, K_color1) -> List[int]:
+    """Host-side checks of a localize request, before anything is launched, with validate_pairs' rules: at least one
+    query, fp32 [P, 3, H, W] or uint8 [P, H, W, 3]; integer ref_idx, one per query, inside the reference bank; the bank's
+    token grid equal to the queries' (the solver needs N x N square); the bank on one device, and the queries there or on
+    the host; K_color0 / K_color1 of shape [P, 3, 3].  Returns ref_idx as a host list."""
+    idx = _host_indices(ref_idx, "ref_idx")
+    if not torch.is_tensor(queries) or queries.dim() != 4:
+        raise MickeyB200Error("queries must be a [P, 3, H, W] float or [P, H, W, 3] uint8 tensor")
+    if queries.dtype == torch.uint8:
+        if queries.shape[-1] != 3:
+            raise MickeyB200Error(f"uint8 queries must be [P, H, W, 3] (HWC, RGB), got {tuple(queries.shape)}")
+        P, H, W = queries.shape[:3]
+    else:
+        if not queries.dtype.is_floating_point or queries.shape[1] != 3:
+            raise MickeyB200Error(f"float queries must be [P, 3, H, W], got {tuple(queries.shape)} {queries.dtype}")
+        P, H, W = queries.shape[0], queries.shape[2], queries.shape[3]
+    if P < 1:
+        raise MickeyB200Error("localize needs at least one query")
+    if len(idx) != P:
+        raise MickeyB200Error(f"ref_idx has {len(idx)} entries for {P} queries: one reference per query")
+    bad = [v for v in idx if not 0 <= v < len(reference)]
+    if bad:
+        raise MickeyB200Error(f"ref_idx {bad[:4]} outside the reference bank of {len(reference)} images")
+    _check_bank(reference)
+    if tuple(reference.grid) != (H // PATCH, W // PATCH):
+        raise MickeyB200Error(f"reference grid {tuple(reference.grid)} differs from the queries' token grid "
+                              f"{(H // PATCH, W // PATCH)} ({H} x {W} images)")
+    devs = {t.device for t in reference.tensors()}
+    if len(devs) != 1:
+        raise MickeyB200Error(f"reference tensors on several devices: {sorted(map(str, devs))}")
+    if queries.device.type != "cpu" and queries.device != reference.device:
+        raise MickeyB200Error(f"queries on {queries.device}, reference on {reference.device}")
+    K0, K1 = torch.as_tensor(K_color0), torch.as_tensor(K_color1)
+    if tuple(K0.shape) != (P, 3, 3) or tuple(K1.shape) != (P, 3, 3):
+        raise MickeyB200Error(f"K_color0 {tuple(K0.shape)} / K_color1 {tuple(K1.shape)} must be [{P}, 3, 3]")
+    return idx
 
 
 def synthetic_backbone_allowed() -> bool:
@@ -470,6 +512,52 @@ class MickeyRelativePose(nn.Module):
         if return_inliers:
             data["inliers_list"] = _inlier_list(st, data["final_scores"], data["kps0"], data["kps1"], data["depth_kp0"],
                                                 data["depth_kp1"])
+        return data
+
+    # -- localization: queries against cached references, the queries alone extracted -----------------------------------
+    @torch.no_grad()
+    def localize(self, reference: MickeyFeatures, ref_idx, queries, K_color0, K_color1, return_inliers: bool = False) -> dict:
+        """Relative pose of P pairs (reference[ref_idx[p]], queries[p]) in one C call (mk_localize): only the queries are
+        extracted, the references' features come from extract_features.
+
+        queries: float [P, 3, H, W] in [0, 1] or uint8 [P, H, W, 3] RGB, on the model's device or on the host (pinned
+        host frames are copied on a side stream, overlapped with the previous call); ref_idx: host list or tensor of P
+        indices into `reference`, whose token grid must be the queries'; K_color0 / K_color1: [P, 3, 3].  Everything is
+        validated on the host (MickeyB200Error before anything is launched or a seed drawn).  Returns the data dict
+        pose_from_features returns for the same pairs, with the same keys and lean_outputs behaviour; one seed is drawn
+        from the torch RNG as in forward(), so under the same seed every output equals forward() on the explicit pairs.
+        Like forward(), it replays a CUDA graph from the third call of a shape on, follows pipeline_depth,
+        assume_inputs_ready and static_outputs, and keeps its own copy of the reference bank for the graph to read
+        (Engine.localize: refreshed when other tensors are passed or theirs change in place)."""
+        idx = validate_localize(reference, ref_idx, queries, K_color0, K_color1)
+        dev = next(self.parameters()).device
+        if reference.device != dev:
+            raise MickeyB200Error(f"reference on {reference.device}, model on {dev}")
+        pool = self._engine_pool()
+        turn = self.__dict__.get("_turn", 0)
+        self.__dict__["_turn"] = turn + 1
+        eng = pool[turn % len(pool)]
+        seed = int(torch.randint(1, 2 ** 62, (1,)).item())
+        bank = tuple(t.float().contiguous() for t in reference.tensors())
+        ridx = torch.tensor(idx, dtype=torch.int32).pin_memory()
+        if queries.dtype != torch.uint8:
+            queries = queries.float()
+        st = eng.localize(bank, ridx, queries, K_color0, K_color1, seed, use_graph=getattr(self, "use_graph", True),
+                          lean=bool(getattr(self, "lean_outputs", False)))
+        static = getattr(self, "static_outputs", False)
+        keep = (lambda t: t) if static else (lambda t: None if t is None else t.clone())   # None: lean_outputs
+        gidx = st["ref_idx"]                             # ref_idx on the device, in the engine's buffer set
+        data = {}
+        _set_correspondences(data, keep(st["kps"]), keep(st["depth"]), (bank[2].index_select(0, gidx), keep(st["scr"])),
+                             (bank[3].index_select(0, gidx), keep(st["dsc"])), reference.grid, self.compute_matches.down_factor,
+                             keep(st["scores"]), keep(st["kp_scores"]))
+        data["final_scores"] = keep(st["final_scores"])
+        data["R"], data["t"], data["inliers"] = _pose_views(keep(st["pose"]))
+        if return_inliers:
+            data["inliers_list"] = _inlier_list(st, data["final_scores"], data["kps0"], data["kps1"], data["depth_kp0"],
+                                                data["depth_kp1"])
+        if not static:
+            eng.release()                                # every read of the static buffers above is queued
         return data
 
     @torch.no_grad()

@@ -15,8 +15,10 @@ random-init weights the poses are noise — the run proves the plumbing and give
 
 Every val/test pair of a scene has the same image0, the scene's reference image.  `--share-reference` reads and extracts
 each reference once (ReferenceBank), extracts only the query images of a step and poses the batch from the two feature
-banks (model.pose_from_features).  The loader then leaves image0 out of its items.  Both paths draw one seed per batch,
-so under the same `--seed` they write the same submission.
+banks (model.pose_from_features).  The loader then leaves image0 out of its items.  `--localize` (implies
+`--share-reference`) poses each batch in one call, model.localize: only the queries are extracted, matched against the
+cached references of the batch's one or two scenes, replayed from a CUDA graph.  Every path draws one seed per batch, so
+under the same `--seed` they write the same submission.
 """
 import argparse
 import json
@@ -82,6 +84,8 @@ def main():
     ap.add_argument("--uint8", action="store_true", help="uint8 HWC batches + fused ingest kernel (a quarter of the H2D bytes)")
     ap.add_argument("--share-reference", action="store_true",
                     help="extract each scene's reference image once and pose every pair from feature banks")
+    ap.add_argument("--localize", action="store_true",
+                    help="with --share-reference: extract only the queries and pose each batch in one call (model.localize)")
     ap.add_argument("--seed", type=int, default=None,
                     help="seed the torch RNG that the solver's per-batch seeds come from (a reproducible submission)")
     ap.add_argument("--output_root", "-o", type=Path, default=Path("results/"))
@@ -112,7 +116,7 @@ def main():
     cfg.TRAINING.NUM_WORKERS = args.workers
     BS = cfg.TRAINING.BATCH_SIZE
 
-    share = args.share_reference
+    share = args.share_reference or args.localize
     dm = DataModule(cfg, drop_last_val=False, uint8_images=args.uint8, pin_memory=True, skip_image0=share)
     loader = dm.val_dataloader() if args.split == "val" else dm.test_dataloader()
     n_pairs = len(loader.dataset)
@@ -154,7 +158,11 @@ def main():
                 data[k] = data[k].to(dev, non_blocking=True)
                 h2d += data[k].numel() * data[k].element_size()
             with torch.no_grad():
-                if share:
+                if args.localize:
+                    banks, idx0 = refs.lookup(list(zip(data["scene_root"], data["pair_names"][0])))
+                    data = model.localize(MickeyFeatures.cat(banks), idx0, data["image1"], data["K_color0"], data["K_color1"])
+                    R, t = data["R"], data["t"]
+                elif share:
                     banks, idx0 = refs.lookup(list(zip(data["scene_root"], data["pair_names"][0])))
                     queries = model.extract_features(data["image1"])
                     data = model.pose_from_features(MickeyFeatures.cat(banks), idx0, queries, range(len(queries)),
@@ -182,7 +190,7 @@ def main():
         args.output_root.mkdir(parents=True, exist_ok=True)
         mksub.save_submission(results, args.output_root / "submission.zip")
         summary = {"pairs": n_pairs, "gpus": world, "batch_size": BS, "steps": n_steps, "wall_s": wall, "pairs_per_s": n_pairs / wall,
-                   "uint8_ingest": bool(args.uint8), "share_reference": share, "h2d_bytes_rank0": h2d, "valid_poses": int(recs[:, 8].sum()),
+                   "uint8_ingest": bool(args.uint8), "share_reference": share, "localize": bool(args.localize), "h2d_bytes_rank0": h2d, "valid_poses": int(recs[:, 8].sum()),
                    "scenes": len(results), "zip": str(args.output_root / "submission.zip")}
         if share:
             summary["references_extracted_rank0"] = refs.extracted
