@@ -21,6 +21,8 @@
 //     dX_i = w_i G_H (Y_i - b) + w_i g_a / (W1 + eps) + c_i R^T r_i,   dY_i = w_i G_H^T (X_i - a) + w_i g_b / (W1 + eps) - c_i r_i
 // with r_i = R X_i + t - Y_i, c_i = dL/dscore * dsigmoid/dd / d_i, g_a = -R^T g_t - G_H (eps b), g_b = g_t - G_H^T (eps a)
 // (eps = 1e-16: sum w_i (Y_i - b) = eps b exactly), and through the back-projection to (u, v, depth).
+// The inlier terms are multiplied by w_i rather than skipped for outliers, so a non-finite G_H (H = 0, rank 1) reaches
+// every entry of the set, as in the autograd tail.
 // Finally each keypoint sums the contributions of the (outer iteration, entry) pairs that drew it in ascending order,
 // one thread per keypoint: no float atomics, so the gradients are the same bits on every run.
 #include <cfloat>
@@ -489,15 +491,16 @@ loss_tail_bwd_kernel(TailArgs A, TailWs W, const float* __restrict__ g_lv, const
       matTvec(R, r, Rtr);
 #pragma unroll
       for (int p = 0; p < 3; ++p) { dX[p] += c * Rtr[p]; dY[p] -= c * r[p]; }
-      if (inlier(A.bits + gh * words, i)) {
-        const double yb[3] = {y[0] - o[HB], y[1] - o[HB + 1], y[2] - o[HB + 2]};
-        const double xa[3] = {x[0] - o[HA], x[1] - o[HA + 1], x[2] - o[HA + 2]};
-        double u[3], v[3];
-        matvec(cf + CGH, yb, u);
-        matTvec(cf + CGH, xa, v);
+      // times w, not under a branch on the bit: a hypothesis whose G_H is not finite (H = 0 or rank 1) makes every
+      // entry of its set non-finite, as torch.svd's backward does in the autograd tail; finite terms add +-0 to outliers
+      const double w = inlier(A.bits + gh * words, i) ? 1.0 : 0.0;
+      const double yb[3] = {y[0] - o[HB], y[1] - o[HB + 1], y[2] - o[HB + 2]};
+      const double xa[3] = {x[0] - o[HA], x[1] - o[HA + 1], x[2] - o[HA + 2]};
+      double u[3], v[3];
+      matvec(cf + CGH, yb, u);
+      matTvec(cf + CGH, xa, v);
 #pragma unroll
-        for (int p = 0; p < 3; ++p) { dX[p] += u[p] + cf[CGA + p]; dY[p] += v[p] + cf[CGB + p]; }
-      }
+      for (int p = 0; p < 3; ++p) { dX[p] += w * (u[p] + cf[CGA + p]); dY[p] += w * (v[p] + cf[CGB + p]); }
     }
     // X = z K^-1 (u, v, 1): du = z dX . Ki[:,0], dv = z dX . Ki[:,1], dz = dX . Ki (u, v, 1)
     const int cell = A.sampled[(long long)s * S + i];
